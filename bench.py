@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the CMGAN hot path on B200 (contract in the task statement).
+"""bench.py -- headline benchmark of the CMGAN hot path on one or more H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--workload train_gd|gen_only]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--workload train_gd|gen_only] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Workload (BASELINE.json configs[2], metric: utterances/sec, 2 s @ 16 kHz): per rank, one step = the reference's whole
@@ -11,7 +11,9 @@ Workload (BASELINE.json configs[2], metric: utterances/sec, 2 s @ 16 kHz): per r
   (one NCCL all-reduce of the flat gradient buffer when N > 1) -> AdamW;
   discriminator: D(clean, est) and D(clean, clean) forward (train mode: spectral-norm power iterations, dropout), loss against a
   fixed synthetic PESQ target (the ``pesq`` package is host code and absent), backward, (all-reduce), AdamW.
-All of it is one CUDA graph per step.  Prints ONE JSON line on rank 0.
+All of it is one CUDA graph per step.  Prints ONE JSON line on rank 0.  ``--dump-outputs DIR`` writes what the last timed step computed
+(losses, enhanced waveforms, parameter gradients) as DIR/<name>.npy; that step starts from the seeded initial state, so two runs or two
+builds can be compared output for output.
 """
 import argparse
 import json
@@ -34,6 +36,7 @@ def emit(obj) -> None:
 
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
@@ -43,7 +46,6 @@ CLIP = 32000
 FWD_GFLOP_PER_UTT = 145.96            # SURVEY.md section 8(d): mm + bmm + conv, 2*MAC, 2 s clip
 STEP_GFLOP_PER_UTT = 3 * FWD_GFLOP_PER_UTT
 TSCB_FWD_GFLOP_PER_UTT = 4 * 19.58    # SURVEY.md section 8(d): four two-stage conformer blocks
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
 
 
 def _peaks():
@@ -51,7 +53,7 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback (H100 SXM data sheet, dense, 700 W)"
 
 
 class ClockSampler:
@@ -123,9 +125,10 @@ def workload_name(B, kind):
 
 # ------------------------------------------------------------------------------------------------ reference arms
 class RefModules:
-    """The reference's own generator / discriminator (unmodified files staged under baseline/_ref by tools/stage_reference.py) driven
-    by the train.py:72-151 glue restated with the torch >= 2 complex STFT API (SURVEY.md section 8c); when the staged files are
-    absent, the oracle port (oracle/cmgan_oracle.py) stands in.  Used by ``--impl reference`` (CPU) and ``gpu_eager_reference``."""
+    """The reference's own generator / discriminator (unmodified files staged under oracle/_ref by oracle/stage_reference.py, which
+    build() runs) driven by the train.py:72-151 glue restated with the torch >= 2 complex STFT API (SURVEY.md section 8c); when the
+    staged files are absent, the oracle port (oracle/cmgan_oracle.py, generator only) stands in and ``kind`` says "port".  Used by
+    ``--impl reference`` (CPU), ``cpu_baseline`` and ``gpu_eager_reference``."""
 
     def __init__(self, device, with_disc=True):
         import torch
@@ -141,6 +144,12 @@ class RefModules:
                     stub = types.ModuleType("pesq")
                     stub.pesq = lambda *a, **k: 0.0
                     sys.modules["pesq"] = stub
+                try:                                    # ... and joblib (for its PESQ batch helper, which the bench never calls either)
+                    import joblib  # noqa: F401
+                except ImportError:
+                    stub = types.ModuleType("joblib")
+                    stub.Parallel = stub.delayed = None
+                    sys.modules["joblib"] = stub
                 sys.path.insert(0, REF_DIR)
                 from models.generator import TSCNet
                 import utils as ref_utils
@@ -241,7 +250,7 @@ def run_reference(args):
     with_disc = args.workload == "train_gd"
     dt, kind = time_cpu(args.steps, args.warmup, with_disc)
     v = 1.0 / dt
-    sample = ("1 utterance (B=1 x 2 s) per step of the workload: " + ("the reference's own TSCNet / Discriminator modules (baseline/_ref)" if kind == "reference"
+    sample = ("1 utterance (B=1 x 2 s) per step of the workload: " + ("the reference's own TSCNet / Discriminator modules (oracle/_ref)" if kind == "reference"
               else "oracle CPU port of the reference") + ", generator forward+backward" + (" + discriminator step" if with_disc and kind == "reference" else "")
               + ", fp32, torch CPU threads = cores")
     emit(({
@@ -280,6 +289,7 @@ def run_ours(args):
     model = cmgan_b200.TSCNet(64, 201).to(dev).train()
     disc = cmgan_b200.Discriminator(16).to(dev).train() if gd else None
     trainer = FusedTrainer(model, disc)          # flat parameter/gradient buffers; rank-0 parameters win (train.py:68)
+    seeded = TrainState(trainer) if args.dump_outputs else None      # the seeded initial state the dumped step starts from
     clean, noisy = synth_batch(B, 1000 + rank, device=dev)
     hclean, hnoisy = synth_batch(B, 1000 + rank, pin=True)
     pesq_t = torch.full((B,), 0.5, device=dev)
@@ -344,12 +354,25 @@ def run_ours(args):
                 trainer.pack.refresh()
         return loss, None
 
+    # With --dump-outputs the LAST timed step starts from the seeded initial state (parameters, optimiser moments and step counts,
+    # BatchNorm / spectral-norm buffers, dropout counter; restored by a few device copies in front of it).  Without the reset the dumped
+    # step would end a training trajectory, and the float atomics of the gradient reductions, whose order varies from run to run, make the
+    # trajectories of two runs drift apart, so that their results could not be compared between runs or builds.
     for _ in range(max(args.warmup, 3)):
         gstep(clean, noisy, pesq_t)
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms = timed(lambda: gstep(clean, noisy, pesq_t), args.steps)
+    last, left = [None], [args.steps]
+
+    def timed_step():
+        left[0] -= 1
+        if args.dump_outputs and left[0] == 0:
+            seeded.restore()
+        last[0] = gstep(clean, noisy, pesq_t)
+    ms = timed(timed_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0], trainer)
     losses = gstep(clean, noisy, pesq_t)
     loss_after = float(losses[0].item())
     dloss_after = float(losses[1].item()) if gd else None
@@ -381,8 +404,9 @@ def run_ours(args):
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong" if args.global_batch else "weak", "vs_baseline": None,
             "dtype": args.precision, "data": "synthetic",
             "config": {"workload": workload_name(B, args.workload), "global_batch": B * world, "clip_samples": CLIP, "parallelism": f"dp{world}",
-                       "l2": "per-step working set (activations saved for backward, several GB) >> 126 MB L2; no explicit flush",
-                       "weights": "torch.manual_seed(0) default init, updated by AdamW every step (lr 5e-4 / 1e-3)", "loss_after": loss_after,
+                       "l2": "per-step working set (activations saved for backward, several GB) >> 50 MB L2; no explicit flush",
+                       "weights": "torch.manual_seed(0) default init, updated by AdamW every step (lr 5e-4 / 1e-3); with --dump-outputs the last "
+                                  "timed step starts again from that init", "loss_after": loss_after,
                        "disc_loss_after": dloss_after,
                        "launch": "one CUDA graph per step (cmgan_b200.trainer.FusedTrainer): forward, losses, backward, "
                                  + ("NCCL gradient all-reduces, " if world > 1 and graph_nccl else "") + "AdamW"
@@ -395,6 +419,8 @@ def run_ours(args):
             "model_tflops": value * STEP_GFLOP_PER_UTT / 1e3,
         }
     if world == 1 and not args.no_extras:
+        last[0] = losses = None
+        trainer.release_graphs()         # the step graph's memory pool: the extra legs capture graphs of their own
         extras(args, out, trainer, model, dev, ms / args.steps)
     if rank == 0:
         emit(out)
@@ -406,14 +432,52 @@ def run_ours(args):
         os._exit(0)
 
 
+class TrainState:
+    """a copy of everything one training step reads and changes besides its inputs: flat parameters, AdamW moments and step counts,
+    module buffers (BatchNorm running statistics, spectral-norm u / v) and the dropout step counter"""
+
+    def __init__(self, trainer):
+        self.trainer = trainer
+        self.flat = [t.clone() for t in self._flat()]
+        self.snap = trainer._snapshot()
+
+    def _flat(self):
+        t = self.trainer
+        return [t.pg, t.opt_g.m, t.opt_g.v] + ([t.pd, t.opt_d.m, t.opt_d.v] if t.disc is not None else [])
+
+    def restore(self) -> None:
+        for dst, src in zip(self._flat(), self.flat):
+            dst.copy_(src)
+        self.trainer._restore(self.snap)
+        if self.trainer.pack is not None:          # the re-tiled weight images follow the parameters
+            self.trainer.pack.refresh()
+
+
+def dump_outputs(out_dir, losses, trainer) -> None:
+    """what the last timed step computed (float32, about 10 MB at the default batch): the generator / discriminator losses, the enhanced
+    waveforms of the batch and the parameter gradients the two AdamW updates consumed.  The updated parameters are not written: AdamW's
+    first step moves every parameter by about lr * sign(gradient), so a parameter whose exact gradient is zero (a bias followed by a
+    normalisation) moves by +-lr depending on the rounding of a sum that is zero in exact arithmetic."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss_g": losses[0], "est_audio": trainer.last["est_audio"], "grads_g": trainer.gg}
+    if losses[1] is not None:
+        arrays["loss_d"] = losses[1]
+        arrays["grads_d"] = trainer.gd
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().reshape(-1).cpu().numpy())
+
+
 def extras(args, out, trainer, model, dev, step_ms):
     """single-GPU explanatory numbers: forward-only (configs[1]), the TSCB stack's roofline, the GEMM family's roofline, the same-box
     GPU-eager reference, the CPU baseline"""
     import torch
     from cmgan_b200 import conformer_block as G, ops, training
     peaks, psrc = _peaks()
-    hbm_peak = peaks.get("hbm_gbs", 6500.0)
-    tf32_peak = peaks.get("bf16_tflops_sustained", 1400.0) / 2.0      # dense tf32 = half the bf16 rate on the same tensor pipe
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)
+    tf32_peak = peaks.get("bf16_tflops_sustained", 989.0) / 2.0      # dense tf32 = half the bf16 rate on the same tensor pipe
 
     def time_graph(fn, reps):
         """capture ``fn`` (after two warm-up passes) and time ``reps`` replays with CUDA events"""
@@ -529,7 +593,7 @@ def extras(args, out, trainer, model, dev, step_ms):
     del probe
     step_s = step_ms * 1e-3
     achieved = b_rows / t_rows / 1e9 if t_rows > 0 else 0.0
-    # The row-parallel GEMM family (tcgen05 tf32): K = 64 .. 256 against N = 64 .. 256 is 13 - 64 flop/byte, far below the ~110 flop/byte
+    # The row-parallel GEMM family (wgmma tf32): K = 64 .. 256 against N = 64 .. 256 is 13 - 64 flop/byte, far below the ~110 flop/byte
     # balance point of tf32 tensor cores vs HBM, so the family is HBM-bound and is reported as such (algorithmic bytes of each launch).
     out["gemm_family"] = {"bound": "hbm", "kernel": "gemm_rows_tc_kernel (every dense contraction of the generator step outside the fused FFN: linear, "
                                                     "pointwise, dilated/strided conv)",
@@ -543,7 +607,7 @@ def extras(args, out, trainer, model, dev, step_ms):
                                     "frac": (b_wg / t_wg / 1e9 / hbm_peak) if t_wg > 0 else 0.0, "share_of_step": t_wg / step_s,
                                     "achieved_tflops": (f_wg / t_wg / 1e12) if t_wg > 0 else 0.0}}
 
-    # ---- the dominant single kernel of the step (profiles/r2_launch_summary.md: 17.6 % of the kernel time, 8 launches): attention backward
+    # ---- a dominant single kernel of the step (8 launches): attention backward
     # dq / dE (attn_bwd_dq_mma_kernel).  Timed alone here, on the bench batch's shapes, both sequence axes (4 launches each per step).
     # Algorithmic flops (SURVEY 8d counts attention as L^2 d MACs per contraction, rel-pos term included): this kernel owns three of the six
     # backward contractions -- dQ = dS K, dQ += dR E, dE = dR^T Q -- = 3 x 2 x 16 = 96 flop per (query, key) pair and head.  It also recomputes
@@ -574,13 +638,8 @@ def extras(args, out, trainer, model, dev, step_ms):
         del qkv, dctx, ctx, lse, delta, dqkv, dE
     dq_t = sum(dq_us) / len(dq_us) * 1e-6                    # average launch duration over the step's 4 + 4 launches
     dq_f = sum(dq_flop) / len(dq_flop)
-    traffic, traffic_note = None, "no ncu capture committed for this batch size"
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(tp):           # dram read + write per launch of the same kernel at the same batch, from the committed ncu launch list
-        tj = json.load(open(tp))
-        if tj.get("batch") == B:
-            traffic, traffic_note = tj.get("traffic_bytes_per_launch"), tj.get("note", "")
-    tf32_burst = peaks.get("bf16_tflops", 1590.0) / 2.0        # kernel timed alone: the burst figure
+    traffic, traffic_note = None, "DRAM traffic per launch not measured"
+    tf32_burst = peaks.get("bf16_tflops", 989.0) / 2.0        # kernel timed alone: the burst figure
     out["roofline"] = {"bound": "tensor", "kernel": "attn_bwd_dq_mma_kernel (attention backward: dQ, dE; mma.sync tf32)", "achieved": dq_f / dq_t / 1e12,
                        "peak": tf32_burst, "unit": "TFLOP/s", "frac": dq_f / dq_t / 1e12 / tf32_burst,
                        "peak_source": f"{psrc}: bf16_tflops (burst, kernel timed alone) / 2 (tf32 runs at half the bf16 rate)",
@@ -590,26 +649,27 @@ def extras(args, out, trainer, model, dev, step_ms):
                        "share_of_step": 4 * (dq_us[0] + dq_us[1]) * 1e-6 / step_s, "algorithmic_gflop_per_launch": dq_f / 1e9,
                        "traffic": traffic, "traffic_note": traffic_note}
 
-    # ---- the same-box competitor (SURVEY 8d / BASELINE.md 4.5): the reference's modules in PyTorch eager on this B200, generator forward +
+    # ---- the same-box competitor (SURVEY 8d / BASELINE.md 4.5): the reference's modules in PyTorch eager on this GPU, generator forward +
     # backward, B = 4, fp32 and with TF32 allowed
     if not args.no_gpu_eager:
         try:
             ref = RefModules(dev, with_disc=False)
             cl, nz = synth_batch(4, 55, device=dev)
             res = {}
-            for name, flag in (("fp32", False), ("tf32", True)):
-                torch.backends.cuda.matmul.allow_tf32 = flag
-                torch.backends.cudnn.allow_tf32 = flag
-                for _ in range(2):
-                    ref.step(cl, nz, False)
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(3):
-                    ref.step(cl, nz, False)
-                e1.record()
-                torch.cuda.synchronize()
-                res[name] = {"value": 4 * 3 / (e0.elapsed_time(e1) * 1e-3), "unit": UNIT, "ms_per_step": e0.elapsed_time(e1) / 3}
+            with torch.device(dev):          # the oracle's own constants (DFT matrices, windows) are created on this GPU too
+                for name, flag in (("fp32", False), ("tf32", True)):
+                    torch.backends.cuda.matmul.allow_tf32 = flag
+                    torch.backends.cudnn.allow_tf32 = flag
+                    for _ in range(2):
+                        ref.step(cl, nz, False)
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(3):
+                        ref.step(cl, nz, False)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    res[name] = {"value": 4 * 3 / (e0.elapsed_time(e1) * 1e-3), "unit": UNIT, "ms_per_step": e0.elapsed_time(e1) / 3}
             torch.backends.cuda.matmul.allow_tf32 = False
             torch.backends.cudnn.allow_tf32 = True
             out["gpu_eager_reference"] = {"kind": ref.kind, "workload": "generator forward + backward (train mode), batch 4 x 2 s, PyTorch eager on this GPU",
@@ -624,7 +684,7 @@ def extras(args, out, trainer, model, dev, step_ms):
         dt, kind = time_cpu(2, 1, with_disc=args.workload == "train_gd")
         out["cpu_baseline"] = {"value": 1.0 / dt, "unit": UNIT, "cores": cores, "kind": kind,
                                "sample": "2 timed steps (after 1 warm-up) of B=1 x 2 s of the same workload through "
-                                         + ("the reference's own modules (baseline/_ref)" if kind == "reference" else "the oracle CPU port") + ", fp32, all host threads"}
+                                         + ("the reference's own modules (oracle/_ref)" if kind == "reference" else "the oracle CPU port") + ", fp32, all host threads"}
 
 
 def main():
@@ -640,9 +700,13 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
     ap.add_argument("--no-gpu-eager", action="store_true", help="skip the GPU-eager reference leg")
     ap.add_argument("--no-extras", action="store_true", help="headline only (no forward-only / roofline / baseline legs)")
-    ap.add_argument("--precision", default="tf32", choices=["tf32", "fp32"], help="dense contractions: tcgen05 tf32 (default) or exact fp32 FFMA")
+    ap.add_argument("--precision", default="tf32", choices=["tf32", "fp32"], help="dense contractions: wgmma tf32 (default) or exact fp32 FFMA")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (losses, enhanced waveforms, parameter gradients) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the results of this project's timed path: not available with --impl reference")
         run_reference(args)
     else:
         run_ours(args)

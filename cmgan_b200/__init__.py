@@ -1,4 +1,4 @@
-"""cmgan_b200: B200-native (sm_100a) hot path of CMGAN behind the reference's nn.Module interface.
+"""cmgan_b200: H100-native (sm_90a) hot path of CMGAN behind the reference's nn.Module interface.
 
     from cmgan_b200 import TSCNet, Discriminator, power_compress, power_uncompress
 

@@ -1,8 +1,8 @@
-"""In-tree build of libcmgan_b200.so (hand-written sm_100a CUDA behind a C ABI).
+"""In-tree build of libcmgan_b200.so (hand-written sm_90a CUDA behind a C ABI).
 
     python -m cmgan_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels with the repo snapshot.
+nvcc cross-compiles without a GPU; the .so and the objects under build/ are git-ignored build products.
 """
 import concurrent.futures
 import hashlib
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcmgan_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

@@ -111,9 +111,9 @@ def conformer_fwd(x, P, p, B, T, F2, axis, training, seed, block_id, sums: _Sums
 
     def ff(xin, name, s1, s2):
         """0.5 * FF(LN(x)) + x  (ref: conformer.py:54-72,136-148,211-212)"""
-        if ops.PRECISION == 1 and ops.FUSED_FFN:
-            # one kernel: the (M, 256) hidden activation lives in TMEM / shared memory only (csrc/ffn_fused.cu); the backward pass
-            # recomputes it from the module input, so nothing but that input is kept
+        if ops.PRECISION == 1:
+            # one kernel: the (M, 256) hidden activation never leaves the SM (csrc/ffn_fused.cu); the backward pass recomputes it from the
+            # module input, so nothing but that input is kept
             W1, W2 = P[f"{p}.{name}.fn.fn.net.0.weight"], P[f"{p}.{name}.fn.fn.net.3.weight"]
             out = _empty(M, C, dev=dev)
             thr, inv = ops.drop_params(dp)
@@ -144,7 +144,7 @@ def conformer_fwd(x, P, p, B, T, F2, axis, training, seed, block_id, sums: _Sums
         gemm(A=xn2, lda=C, W=Wkv, sb_k=1, sb_n=C, C=(qkv, C), ldc=3 * C, M=M, N=2 * C, Cin=C)
     ctx = _empty(M, C, dev=dev)
     lse = _empty(M, 4, dev=dev)
-    call(("cmgan_attention_fwd_tc" if ops.ATTN_TC else "cmgan_attention_fwd_tf32") if ops.PRECISION == 1 else "cmgan_attention_fwd", qkv, P[f"{p}.attn.fn.rel_pos_emb.weight"], B, T, F2, axis,
+    call("cmgan_attention_fwd_tf32" if ops.PRECISION == 1 else "cmgan_attention_fwd", qkv, P[f"{p}.attn.fn.rel_pos_emb.weight"], B, T, F2, axis,
          ctx, lse)
     x2 = _empty(M, C, dev=dev)
     gemm(A=ctx, lda=C, W=P[f"{p}.attn.fn.to_out.weight"], sb_k=1, sb_n=C, bias=P[f"{p}.attn.fn.to_out.bias"], C=x2, ldc=C, M=M, N=C, Cin=C,
@@ -203,14 +203,15 @@ def conformer_bwd(dy, S: dict, P, G: Dict[str, torch.Tensor], B, T, F2, sums: _S
         # out = xin + 0.5 * drop2(W2 a + b2),  a = swish(h) * drop1,  h = W1 LN(xin) + b1;   dz = 0.5 * drop2-mask * dout
         W1, W2 = P[f"{p}.{name}.fn.fn.net.0.weight"], P[f"{p}.{name}.fn.fn.net.3.weight"]
         if f.get("fused"):
-            # one kernel for the data gradients (hidden activation recomputed, LayerNorm backward in its epilogue); it leaves the operands
-            # of the two weight-gradient GEMMs behind: a = swish(h) * drop, dh, xn
+            # hidden activation recomputed, dh formed in the same kernel; it leaves the operands of the two weight-gradient GEMMs behind:
+            # a = swish(h) * drop, dh, xn
             a, dh, xn, dxv = _empty(M, 4 * C, dev=dev), _empty(M, 4 * C, dev=dev), _empty(M, C, dev=dev), _empty(M, C, dev=dev)
+            ws = _empty(M * (2 + C), dev=dev)
             thr, inv = ops.drop_params(dp)
             call("cmgan_ffn_bwd", xin, C, dz, C, dout, C, res2, C if res2 is not None else 0, M, P[f"{p}.{name}.fn.norm.weight"],
                  P[f"{p}.{name}.fn.norm.bias"], ops.packed_weight(W1, 0, 1, C, C, 1, 4 * C), P[f"{p}.{name}.fn.fn.net.0.bias"],
                  ops.packed_weight(W2, 0, 4 * C, 1, C, 1, 4 * C), ops.packed_weight(W1, 0, C, 1, 4 * C, 1, C), s1 & 0xFFFFFFFFFFFFFFFF, thr, inv,
-                 ops.SEED_DEV, dxv, C, a, dh, xn, G[f"{p}.{name}.fn.norm.weight"], G[f"{p}.{name}.fn.norm.bias"])
+                 ops.SEED_DEV, dxv, C, a, dh, xn, G[f"{p}.{name}.fn.norm.weight"], G[f"{p}.{name}.fn.norm.bias"], ws)
             gemm(wgrad=True, A=a, lda=4 * C, Cin=4 * C, D=dz, ldd=C, N=C, W=None, C=G[f"{p}.{name}.fn.fn.net.3.weight"], sb_k=1, sb_n=4 * C, ldc=0,
                  M=M, dbias=G[f"{p}.{name}.fn.fn.net.3.bias"])
             gemm(wgrad=True, A=xn, lda=C, Cin=C, D=dh, ldd=4 * C, N=4 * C, W=None, C=G[f"{p}.{name}.fn.fn.net.0.weight"], sb_k=1, sb_n=C, ldc=0, M=M,

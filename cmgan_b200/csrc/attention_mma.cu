@@ -718,7 +718,7 @@ CMGAN_API int cmgan_attention_fwd_tf32_nbuf(const float* qkv, const float* E, in
 // scratch (optional, cmgan_attention_bwd_ws_floats): block-private dE accumulators in global memory -> the dq kernel needs 60 KB instead of
 // 110+ KB of shared memory and runs 3 blocks / SM (any L) instead of 2 (1 at L = 1281).
 static int dq_blocks(int ntile, int per_sm, int n_items) {
-    int ng = (148 * per_sm) / ntile;
+    int ng = (cmgan_num_sms() * per_sm) / ntile;
     if (ng < 1) ng = 1;
     return ng > n_items ? n_items : ng;
 }

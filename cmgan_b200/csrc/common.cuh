@@ -1,4 +1,4 @@
-// Shared device/host helpers for the cmgan_b200 kernels (sm_100a).
+// Shared device/host helpers for the cmgan_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,6 +10,7 @@
 // ---- error channel --------------------------------------------------------------------------------
 void cmgan_set_error(const char* fmt, ...);
 int cmgan_check_launch(const char* what);   // cudaGetLastError() -> 0 / -1 (+ message)
+int cmgan_num_sms();                         // multiprocessors of the current device (queried once)
 
 #define CMGAN_REQUIRE(cond, ...)                       \
     do {                                               \

@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(256, 2) glu_dwconv_bwd_kernel(const float* __r
 }
 
 int resident_grid(long total, int per_sm) {
-    const long slots = 148L * per_sm;
+    const long slots = (long)cmgan_num_sms() * per_sm;
     return (int)(total < slots ? total : slots);
 }
 

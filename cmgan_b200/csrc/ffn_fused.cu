@@ -1,881 +1,287 @@
-// Fused macaron feed-forward of the conformer block (reference conformer.py:54-72,136-148,211-212) for sm_100a:
+// Fused macaron feed-forward of the conformer block (reference conformer.py:54-72,136-148,211-212) for sm_90a:
 //
 //     out = x + alpha * drop2( W2 ( swish(W1 LN(x) + b1) * drop1 ) + b2 )                alpha = 0.5, C = 64, hidden = 256
 //
-// ONE kernel per feed-forward: a persistent CTA per SM walks 128-row tiles; the (128 x 256) hidden tile never leaves the SM --
-// it is born in TMEM (tcgen05.mma, tf32 operands, fp32 accumulation), activated in registers and handed to the second
-// contraction through a ring of K-major SWIZZLE_128B shared-memory chunks; both weight matrices (2 x 64 KB of pre-tiled tf32)
-// stay resident in shared memory for the CTA's lifetime.  HBM traffic is the compulsory read of x and write of out.
+// Forward: ONE kernel.  A persistent CTA (one warpgroup) per SM keeps both pre-tiled tf32 weight images (2 x 64 KB, K-major
+// SWIZZLE_128B) in shared memory and walks 64-row tiles: LayerNorm (two threads per row) -> the normalised tile as the A operand ->
+// wgmma into a 64 x 256 register accumulator -> bias, Swish, dropout, tf32 rounding -> the hidden tile as the A operand of the second
+// contraction (64 KB of shared memory; it never reaches HBM) -> wgmma into 64 x 64 -> bias, dropout, alpha, residual -> store.
+// Only the module input is kept for the backward pass.
 //
-//   warps 0-3   LayerNorm producers (thread = row): load x (one tile ahead of the tensor pipe), LayerNorm in registers (no shuffles),
-//               write the normalised tf32 row into the K-major A tile.
-//   last 8      output epilogue (thread = half a row): residual prefetched from L2, acc2 from TMEM, bias, dropout, alpha, store.
-//   warp 4      TMEM allocation; one lane issues every tcgen05.mma / tcgen05.commit:
-//                 GEMM1  H[:, 64 q .. 64 q + 63] = xn W1^T in four N = 64 quarters (the activation warps start on quarter 0 while
-//                        quarters 1-3 are still in the tensor pipe; quarter q of the NEXT tile is issued as soon as the activation
-//                        warps have drained quarter q of this one),
-//                 GEMM2  acc2 += a_chunk W2_chunk^T over eight K = 32 chunks as they arrive in the ring (double-buffered accumulator).
-//   warp 5      weight images -> shared memory by cp.async.bulk, once.
-//   warps 6-13  activation (2 groups x 4 lane quarters, chunks round-robin): tcgen05.ld 32 columns of H -> + b1 -> swish -> counter-based dropout -> round to tf32 -> st.shared into
-//               the ring slot in the UMMA K-major swizzled layout -> fence.proxy.async -> mbarrier.
-// All mbarrier waits are bounded (tc_ptx.cuh): a protocol bug traps instead of hanging the GPU.
-#include <cuda.h>      // CUtensorMap (types only; the encoder is fetched from the driver at run time)
+// Backward: one kernel recomputes the hidden pre-activation h (LN + first contraction) and forms dh = (dz W2) * swish'(h) * drop1 one
+// 64-column quarter of the hidden layer at a time (two 64 x 64 accumulators in registers), writing the operands of the two weight-gradient
+// GEMMs (xn, a = swish(h) * drop1, dh) and the LayerNorm statistics; the data gradient dLN = dh W1 and the LayerNorm backward then run
+// as the library's row GEMM and LayerNorm-backward kernels.
+// Dropout masks are the counter-based hash of the GEMM epilogues (csrc/gemm_tc.cu): pair (m * N + n) / 2, 16 bits per element.
+#include <cstring>
 
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
+#include "gemm_args.h"
 #include "tc_ptx.cuh"
+
+int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st);    // gemm_tc.cu
 
 namespace {
 using namespace cmgan_tc;
 
-constexpr int BM = 128, C = 64, HID = 256;
-constexpr int CHUNK_BYTES = BM * 128;                 // 128 rows x 32 floats (one 128-byte swizzle row per matrix row) = 16 KB
-constexpr int W1_BYTES = 2 * HID * 128;               // 2 K-chunks x 256 rows x 128 B = 64 KB
-constexpr int W2_BYTES = 8 * C * 128;                 // 8 K-chunks x  64 rows x 128 B = 64 KB
-constexpr int XN_BYTES = 2 * CHUNK_BYTES;             // A tile of GEMM1: 128 x 64
-constexpr int RING = 3;                               // hidden chunks in flight between the activation warps and GEMM2
-constexpr int NACT_GROUPS = 2;                        // activation groups of 4 warps (one per TMEM lane quarter), chunks round-robin
-constexpr int NEPI = 8;                               // output warps: two per TMEM lane quarter, 32 of the 64 columns each
-constexpr int NTHREADS = 32 * (6 + 4 * NACT_GROUPS + NEPI);      // 4 LayerNorm + MMA + weights + activation + output warps
-constexpr int TMEM_COLS = 512;                        // H: 4 x 64, acc2: 2 x 64
-constexpr int SMEM_FWD = 1024 + W1_BYTES + W2_BYTES + XN_BYTES + RING * CHUNK_BYTES + 2048;
+constexpr int BM = 64, C = 64, HID = 256, NT = 128;
+constexpr int CHUNK = BM * 128;                 // 64 rows x 32 floats = 8 KB
+constexpr int W_BYTES = 64 * 1024;              // one packed 64 x 256 weight image
+
+// byte offset of (row r, float column c of a 32-float chunk) in a K-major SWIZZLE_128B chunk
+__device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 2) ^ r) & 7) << 4) + (c & 3) * 4); }
+
+// dropout scales of the element pair (m, n), (m, n + 1), n even
+__device__ __forceinline__ float2 drop_pair(long m, int n, int N, uint32_t seed32, uint32_t thr16, float inv_keep, bool on) {
+    if (!on) return make_float2(1.f, 1.f);
+    const uint32_t pr = (uint32_t)(((unsigned long long)m * (unsigned long long)N + (unsigned long long)n) >> 1);
+    const uint32_t h = cmgan_mix32((pr * 0x9E3779B1u) ^ seed32);
+    return make_float2((h & 0xFFFFu) >= thr16 ? inv_keep : 0.f, (h >> 16) >= thr16 ? inv_keep : 0.f);
+}
+
+__device__ __forceinline__ void copy_image(uint8_t* dst, const float* src, int bytes) {
+    const uint4* s = reinterpret_cast<const uint4*>(src);
+    uint4* d = reinterpret_cast<uint4*>(dst);
+    for (int i = threadIdx.x; i < bytes / 16; i += NT) d[i] = __ldg(s + i);
+}
+
+// LayerNorm of the tile's rows (two threads per row, 32 channels each) -> tf32 A operand (2 chunks); rows past M are zero.
+// Returns (mean, rstd) of the thread's row.
+__device__ __forceinline__ float2 ln_tile(const float* __restrict__ x, long ldx, long m0, long M, const float* __restrict__ g,
+                                          const float* __restrict__ b, uint8_t* sXn, float* xn_out) {
+    const int r = threadIdx.x >> 1, half = threadIdx.x & 1;
+    const long m = m0 + r;
+    float v[32];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        float4 t = m < M ? __ldg(reinterpret_cast<const float4*>(x + m * ldx + half * 32 + 4 * q)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s += v[i];
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    const float mean = s * (1.f / C);
+    float q2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { const float d = v[i] - mean; q2 += d * d; }
+    q2 += __shfl_xor_sync(0xffffffffu, q2, 1);
+    const float rstd = rsqrtf(q2 * (1.f / C) + 1e-5f);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        float o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int c = half * 32 + 4 * q + j;
+            o[j] = m < M ? to_tf32((v[4 * q + j] - mean) * rstd * __ldg(g + c) + __ldg(b + c)) : 0.f;
+        }
+        *reinterpret_cast<float4*>(sXn + half * CHUNK + swz(r, 4 * q)) = make_float4(o[0], o[1], o[2], o[3]);
+        if (xn_out && m < M) *reinterpret_cast<float4*>(xn_out + m * C + half * 32 + 4 * q) = make_float4(o[0], o[1], o[2], o[3]);
+    }
+    return make_float2(mean, rstd);
+}
 
 struct FfnFwdArgs {
-    const float* x; long long ldx;
-    float* out; long long ldo;
-    const float* ln_g; const float* ln_b;
-    const float* W1p; const float* b1;
-    const float* W2p; const float* b2;
-    long long M;
-    float alpha;
-    unsigned long long seed1, seed2; unsigned int thr; float inv_keep;
-    const unsigned long long* seed_dev;
-    long long* dbg;                  // optional timeline (CTA 0): clock64 stamps, 64 per warp (tools/bench_ffn.py --timeline)
+    const float* x; long long ldx; float* out; long long ldo;
+    const float* ln_g; const float* ln_b; const float* W1p; const float* b1; const float* W2p; const float* b2;
+    long long M; float alpha; unsigned long long seed1, seed2; unsigned int thr; float inv_keep; const unsigned long long* seed_dev;
 };
 
-// byte offset of (row r, 16-byte unit c of the row's 128 bytes) inside a K-major SWIZZLE_128B chunk
-__device__ __forceinline__ uint32_t sw_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, float a, float b, float c, float d) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-#define FFN_STAMP(slot)                                                                                   \
-    do {                                                                                                  \
-        if (g.dbg && blockIdx.x == 0 && lane == 0 && (slot) < 64) g.dbg[warp * 64 + (slot)] = clock64();  \
-    } while (0)
-
-__global__ void __launch_bounds__(NTHREADS, 1) ffn_fwd_kernel(const __grid_constant__ FfnFwdArgs g) {
+__global__ void __launch_bounds__(NT, 1) ffn_fwd_kernel(const __grid_constant__ FfnFwdArgs g) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t sW1 = base, sW2 = sW1 + W1_BYTES, sXn = sW2 + W2_BYTES, sRing = sXn + XN_BYTES;
-    const uint32_t sPar = sRing + RING * CHUNK_BYTES;            // gamma[64] beta[64] b2[64] b1[256] floats = 1792 B
-    float* par = reinterpret_cast<float*>(base_ptr + (sPar - base));
-    const uint32_t bars = sPar + 1792;
-    const uint32_t xn_full = bars, xn_empty = bars + 8, wready = bars + 16;
-    auto hq_full = [&](int q) { return bars + 24u + 8u * q; };                   // [4]
-    auto hid_full = [&](int s) { return bars + 56u + 8u * s; };                  // [RING]
-    auto hid_empty = [&](int s) { return bars + 56u + 8u * (RING + s); };        // [RING]
-    auto acc_full = [&](int b) { return bars + 56u + 16u * RING + 8u * b; };     // [2]
-    auto acc_empty = [&](int b) { return bars + 72u + 16u * RING + 8u * b; };    // [2]
-    const uint32_t tmem_ptr_addr = bars + 88u + 16u * RING;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ntiles = (int)((g.M + BM - 1) / BM);
-    const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-
-    if (tid == 0) {
-        mbar_init(xn_full, 4); mbar_init(xn_empty, 1); mbar_init(wready, 1);
-        for (int q = 0; q < 4; ++q) mbar_init(hq_full(q), 1);
-        for (int s = 0; s < RING; ++s) { mbar_init(hid_full(s), 4); mbar_init(hid_empty(s), 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(acc_full(b), 1); mbar_init(acc_empty(b), NEPI); }
-        fence_barrier_init();
-    }
-    for (int i = tid; i < 448; i += NTHREADS)
-        par[i] = i < 64 ? __ldg(g.ln_g + i) : i < 128 ? __ldg(g.ln_b + i - 64) : i < 192 ? __ldg(g.b2 + i - 128) : __ldg(g.b1 + i - 192);
-    if (warp == 4) tmem_alloc(tmem_ptr_addr, TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_addr));
-    const float* gam = par; const float* bet = par + 64; const float* b2s = par + 128; const float* b1s = par + 192;
-
-    if (warp < 4) {
-        // ================================ LayerNorm producers ================================
-        for (int lt = 0; lt < my_tiles; ++lt) {
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + tid;
-            float v[64];
-            if (row < g.M) {
-                const float4* xr = reinterpret_cast<const float4*>(g.x + row * g.ldx);
+    uint8_t* const bp = smem_raw + (base - smem_u32(smem_raw));
+    uint8_t* const sW1 = bp;                       // 2 chunks x 256 rows
+    uint8_t* const sW2 = bp + W_BYTES;             // 8 chunks x 64 rows
+    uint8_t* const sXn = bp + 2 * W_BYTES;         // 2 chunks x 64 rows
+    uint8_t* const sH = sXn + 2 * CHUNK;           // 8 chunks x 64 rows
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, fg = lane >> 2, ft = lane & 3;
+    const bool drop_on = g.thr != 0u;
+    const uint32_t thr16 = g.thr >> 16;
+    const uint32_t s1 = cmgan_seed32(cmgan_eff_seed(g.seed1, g.seed_dev)), s2 = cmgan_seed32(cmgan_eff_seed(g.seed2, g.seed_dev));
+    copy_image(sW1, g.W1p, W_BYTES);
+    copy_image(sW2, g.W2p, W_BYTES);
+    const long ntiles = (g.M + BM - 1) / BM;
+    for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long m0 = tile * BM;
+        ln_tile(g.x, g.ldx, m0, g.M, g.ln_g, g.ln_b, sXn, nullptr);
+        fence_proxy_async();
+        __syncthreads();
+        float acc[16][8];
+        wgmma_fence();
+        mma_chunk<16, 16>(acc, gmma_desc_sw128(base + 2 * W_BYTES), gmma_desc_sw128(base), true);
+        mma_chunk<16, 16>(acc, gmma_desc_sw128(base + 2 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128), false);
+        wgmma_commit();
+        wgmma_wait<0>();
+        // hidden activation -> second A operand (fragment rows 16 warp + fg (+ 8), columns 16 j + 8 i + 2 ft (+ 1))
 #pragma unroll
-                for (int c4 = 0; c4 < 16; ++c4) { const float4 t = __ldg(xr + c4); v[4 * c4] = t.x; v[4 * c4 + 1] = t.y; v[4 * c4 + 2] = t.z; v[4 * c4 + 3] = t.w; }
-            } else {
+        for (int j = 0; j < 16; ++j)
 #pragma unroll
-                for (int k = 0; k < 64; ++k) v[k] = 0.f;
-            }
-            float s = 0.f;
+            for (int i = 0; i < 2; ++i)
 #pragma unroll
-            for (int k = 0; k < 64; ++k) s += v[k];
-            const float mean = s * (1.f / 64.f);
-            float q = 0.f;
-#pragma unroll
-            for (int k = 0; k < 64; ++k) { const float d = v[k] - mean; q = fmaf(d, d, q); }
-            const float rstd = rsqrtf(q * (1.f / 64.f) + 1e-5f);
-            FFN_STAMP(3 * lt);
-            mbar_wait(xn_empty, (uint32_t)((lt & 1) ^ 1));          // GEMM1 of the previous tile has read the A tile
-            FFN_STAMP(3 * lt + 1);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) {
-                float o[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) o[j] = to_tf32(fmaf((v[4 * c + j] - mean) * rstd, gam[4 * c + j], bet[4 * c + j]));
-                st_shared_v4(sXn + (uint32_t)(c >> 3) * CHUNK_BYTES + sw_off(tid, c & 7), o[0], o[1], o[2], o[3]);
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(xn_full);
-            FFN_STAMP(3 * lt + 2);
-        }
-    } else if (warp >= 6 + 4 * NACT_GROUPS) {
-        // ================================ output epilogue (last NEPI warps) ================================
-        // thread = half a row (32 columns).  The residual half row is requested BEFORE the wait for the accumulator, so its L2 latency
-        // (the row was read by this CTA one tile ago) hides behind the tile's second contraction instead of serialising behind it.
-        const int ew = warp - (6 + 4 * NACT_GROUPS);
-        const int lq = warp & 3;                    // TMEM lane quarter
-        const int hv = ew >> 2;                     // column half
-        const int rloc = lq * 32 + lane;
-        const uint32_t seed2_32 = cmgan_seed32(cmgan_eff_seed(g.seed2, g.seed_dev));
-        const uint32_t thr16 = g.thr >> 16;
-        const bool drop_on = g.thr != 0u;
-        for (int lt = 0; lt < my_tiles; ++lt) {
-            const int buf = lt & 1;
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + rloc;
-            const bool ok = row < g.M;
-            float4 xv[8];
-            if (ok) {
-                const float4* xr = reinterpret_cast<const float4*>(g.x + row * g.ldx) + hv * 8;
-#pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) xv[c4] = __ldg(xr + c4);
-            }
-            FFN_STAMP(3 * lt);
-            mbar_wait(acc_full(buf), (uint32_t)((lt >> 1) & 1));
-            FFN_STAMP(3 * lt + 1);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + (uint32_t)(HID + buf * C + hv * 32) + ((uint32_t)(lq * 32) << 16);
-            float r[32];
-            tmem_ld16f_nowait(taddr, r); tmem_ld16f_nowait(taddr + 16, r + 16);
-            tmem_wait_ld();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty(buf));
-            if (ok) {
-                float4* orow = reinterpret_cast<float4*>(g.out + row * g.ldo) + hv * 8;
-                const uint32_t pair0 = (uint32_t)(((unsigned long long)row * C + (unsigned long long)(hv * 32)) >> 1);
-#pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) {
-                    float ds[4] = {1.f, 1.f, 1.f, 1.f};
-                    if (drop_on) {
-                        const uint32_t pr = pair0 + 2u * c4;
-                        const uint32_t h0 = cmgan_mix32((pr * 0x9E3779B1u) ^ seed2_32), h1 = cmgan_mix32(((pr + 1u) * 0x9E3779B1u) ^ seed2_32);
-                        ds[0] = (h0 & 0xFFFFu) >= thr16 ? g.inv_keep : 0.f; ds[1] = (h0 >> 16) >= thr16 ? g.inv_keep : 0.f;
-                        ds[2] = (h1 & 0xFFFFu) >= thr16 ? g.inv_keep : 0.f; ds[3] = (h1 >> 16) >= thr16 ? g.inv_keep : 0.f;
-                    }
-                    const int k = hv * 32 + 4 * c4;
-                    float4 o;
-                    o.x = fmaf(g.alpha * ds[0], r[4 * c4 + 0] + b2s[k + 0], xv[c4].x);
-                    o.y = fmaf(g.alpha * ds[1], r[4 * c4 + 1] + b2s[k + 1], xv[c4].y);
-                    o.z = fmaf(g.alpha * ds[2], r[4 * c4 + 2] + b2s[k + 2], xv[c4].z);
-                    o.w = fmaf(g.alpha * ds[3], r[4 * c4 + 3] + b2s[k + 3], xv[c4].w);
-                    orow[c4] = o;
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int r = 16 * warp + fg + 8 * hh, n = 16 * j + 8 * i + 2 * ft;
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b1 + n));
+                    const float2 ds = drop_pair(m0 + r, n, HID, s1, thr16, g.inv_keep, drop_on);
+                    const float h0 = acc[j][4 * i + 2 * hh] + bb.x, h1 = acc[j][4 * i + 2 * hh + 1] + bb.y;
+                    *reinterpret_cast<float2*>(sH + (n >> 5) * CHUNK + swz(r, n & 31)) =
+                        make_float2(to_tf32(swishf_(h0) * ds.x), to_tf32(swishf_(h1) * ds.y));
                 }
-            }
-            FFN_STAMP(3 * lt + 2);
-        }
-    } else if (warp == 4) {
-        // ================================ MMA issuer ================================
-        if (lane == 0 && my_tiles > 0) {
-            const uint32_t idesc64 = make_idesc_tf32(BM, 64, 0, 0);
-            mbar_wait(wready, 0);
-            auto issue_h_quarter = [&](int lt, int q, bool block) -> bool {     // H[:, 64 q ..] of tile lt (xn of that tile is in the A tile)
-                if (q == 0) {
-                    if (block) mbar_wait(xn_full, (uint32_t)(lt & 1));
-                    else if (!mbar_test(xn_full, (uint32_t)(lt & 1))) return false;
-                    tc_fence_after();
+        fence_proxy_async();
+        __syncthreads();
+        float acc2[4][8];
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+            mma_chunk<4, 4>(acc2, gmma_desc_sw128(base + 2 * W_BYTES + 2 * CHUNK + c * CHUNK), gmma_desc_sw128(base + W_BYTES + c * CHUNK), c == 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const long m = m0 + 16 * warp + fg + 8 * hh;
+                    if (m >= g.M) continue;
+                    const int n = 16 * j + 8 * i + 2 * ft;
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b2 + n));
+                    const float2 ds = drop_pair(m, n, C, s2, thr16, g.inv_keep, drop_on);
+                    const float2 xr = __ldg(reinterpret_cast<const float2*>(g.x + m * g.ldx + n));
+                    *reinterpret_cast<float2*>(g.out + m * g.ldo + n) =
+                        make_float2(xr.x + g.alpha * (acc2[j][4 * i + 2 * hh] + bb.x) * ds.x, xr.y + g.alpha * (acc2[j][4 * i + 2 * hh + 1] + bb.y) * ds.y);
                 }
-#pragma unroll
-                for (int kc = 0; kc < 2; ++kc) {
-                    const uint64_t adesc = make_desc_sw128(sXn + kc * CHUNK_BYTES, 16, 1024);
-                    const uint64_t bdesc = make_desc_sw128(sW1 + kc * (HID * 128) + q * (64 * 128), 16, 1024);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_tf32(tmem_base + (uint32_t)(q * 64), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc64, (kc | k) != 0 ? 1u : 0u);
-                }
-                umma_commit(hq_full(q));
-                if (q == 3) umma_commit(xn_empty);
-                return true;
-            };
-            for (int q = 0; q < 4; ++q) issue_h_quarter(0, q, true);
-            for (int lt = 0; lt < my_tiles; ++lt) {
-                const int buf = lt & 1;
-                const bool more = lt + 1 < my_tiles;
-                int hq_next = 0;                                   // quarters of tile lt + 1 already in the tensor pipe
-                mbar_wait(acc_empty(buf), (uint32_t)(((lt >> 1) & 1) ^ 1));      // output epilogue of tile lt - 2 has drained this accumulator
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + (uint32_t)(HID + buf * C);
-                for (int j = 0; j < 8; ++j) {
-                    const long gch = (long)lt * 8 + j;
-                    const int s = (int)(gch % RING);
-                    mbar_wait(hid_full(s), (uint32_t)((gch / RING) & 1));
-                    FFN_STAMP((int)gch);
-                    tc_fence_after();
-                    const uint64_t adesc = make_desc_sw128(sRing + s * CHUNK_BYTES, 16, 1024);
-                    const uint64_t bdesc = make_desc_sw128(sW2 + j * (C * 128), 16, 1024);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_tf32(tacc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc64, (j | k) != 0 ? 1u : 0u);
-                    umma_commit(hid_empty(s));
-                    // chunk 2 q + 1 in the ring means the activation warps have finished reading quarter q of H: refill it for the next tile,
-                    // but never stall GEMM2 on the LayerNorm producers (probe, do not wait)
-                    while (more && hq_next < ((j + 1) >> 1)) {
-                        if (!issue_h_quarter(lt + 1, hq_next, false)) break;
-                        ++hq_next;
-                    }
-                }
-                umma_commit(acc_full(buf));
-                while (more && hq_next < 4) { issue_h_quarter(lt + 1, hq_next, true); ++hq_next; }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 5) {
-        if (lane == 0) {
-            mbar_arrive_expect_tx(wready, (uint32_t)(W1_BYTES + W2_BYTES));
-            for (int i = 0; i < 4; ++i) bulk_g2s(sW1 + i * (W1_BYTES / 4), g.W1p + (long)i * (W1_BYTES / 16), (uint32_t)(W1_BYTES / 4), wready);
-            for (int i = 0; i < 4; ++i) bulk_g2s(sW2 + i * (W2_BYTES / 4), g.W2p + (long)i * (W2_BYTES / 16), (uint32_t)(W2_BYTES / 4), wready);
-        }
-        __syncwarp();
-    } else if (warp >= 6) {
-        // ================================ activation warps ================================
-        // group g (4 warps, one per TMEM lane quarter) takes hidden chunks g, g + NACT_GROUPS, ... of the CTA's chunk stream (8 per tile)
-        const int lq = warp & 3;                    // TMEM lane quarter this warp may touch
-        const int grp = (warp - 6) >> 2;
-        const int rloc = lq * 32 + lane;            // row within the tile
-        const uint32_t seed1_32 = cmgan_seed32(cmgan_eff_seed(g.seed1, g.seed_dev));
-        const uint32_t thr16 = g.thr >> 16;
-        const bool drop_on = g.thr != 0u;
-        const long nchunks = 8L * my_tiles;
-        for (long gch = grp; gch < nchunks; gch += NACT_GROUPS) {
-            const int sl = (int)(gch % RING);
-            const uint32_t dst = sRing + sl * CHUNK_BYTES;
-            const int lt = (int)(gch >> 3), j = (int)(gch & 7), q = j >> 1;
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + rloc;
-            const int n0 = j * 32;
-            const int ck = (int)(gch / NACT_GROUPS);
-            FFN_STAMP(4 * ck);
-            mbar_wait(hq_full(q), (uint32_t)(lt & 1));
-            FFN_STAMP(4 * ck + 1);
-            tc_fence_after();
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + (uint32_t)n0 + ((uint32_t)(lq * 32) << 16);
-            tmem_ld16_nowait(taddr, r); tmem_ld16_nowait(taddr + 16, r + 16);
-            tmem_wait_ld();
-            float a[32];
-            const uint32_t pair0 = (uint32_t)(((unsigned long long)row * HID + (unsigned long long)n0) >> 1);
-#pragma unroll
-            for (int p = 0; p < 16; ++p) {
-                float d0 = 1.f, d1 = 1.f;
-                if (drop_on) {
-                    const uint32_t h = cmgan_mix32(((pair0 + (uint32_t)p) * 0x9E3779B1u) ^ seed1_32);
-                    d0 = (h & 0xFFFFu) >= thr16 ? g.inv_keep : 0.f; d1 = (h >> 16) >= thr16 ? g.inv_keep : 0.f;
-                }
-                const float v0 = __uint_as_float(r[2 * p]) + b1s[n0 + 2 * p], v1 = __uint_as_float(r[2 * p + 1]) + b1s[n0 + 2 * p + 1];
-                a[2 * p] = to_tf32(swishf_(v0) * d0);
-                a[2 * p + 1] = to_tf32(swishf_(v1) * d1);
-            }
-            FFN_STAMP(4 * ck + 2);
-            mbar_wait(hid_empty(sl), (uint32_t)(((gch / RING) & 1) ^ 1));
-#pragma unroll
-            for (int c = 0; c < 8; ++c) st_shared_v4(dst + sw_off(rloc, c), a[4 * c], a[4 * c + 1], a[4 * c + 2], a[4 * c + 3]);
-            fence_proxy_async();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(hid_full(sl));
-            FFN_STAMP(4 * ck + 3);
-        }
-    }
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
+        __syncthreads();          // sXn / sH are rewritten by the next tile
     }
 }
-
-
-// =====================================================================================================================================
-// Backward of the feed-forward module in one kernel (data gradients; the two weight-gradient GEMMs read what it writes):
-//
-//     xn = LN(x);  h = xn W1^T + b1;  s = sigmoid(h);  a = h s m1;                      (recomputed: the forward pass saved only x)
-//     da = dz W2;  dh = da m1 s (1 + h (1 - s));  dxn = dh W1;  dx = LNbwd(dxn) + dout (+ res2);  dgamma, dbeta
-//
-// with dz = alpha * m2 * dout materialised by the producer of dout.  Outputs for the weight gradients: a, dh (M, 256), xn (M, 64), all
-// rounded to tf32.  Per 128-row tile: H and DA are born in TMEM quarter by quarter (64 hidden columns), the activation warps turn them
-// into a / dh chunks in two K-major shared-memory rings; the dh ring feeds the third contraction (accumulator double-buffered in TMEM)
-// and BOTH rings are written to HBM by TMA (cp.async.bulk.tensor stores un-swizzle them into row-major (M, 256)): the activation warps
-// never touch global memory.  The epilogue warps (thread = half a row, inputs prefetched before the accumulator is ready) run the
-// LayerNorm backward straight from TMEM.
-// Shared memory (fp32 operands are fat): no weight is resident -- W1 (for H), W2 (for DA) and W1 in its K = hidden form (for dxn) stream
-// through three 8 KB slots each (192 KB per tile out of L2), which leaves room for separate xn and dz A tiles (the next tile's H / DA
-// quarters are issued while this tile's are still being consumed) and for the two output rings.
-//   warps 0-3    row producers: x -> LayerNorm -> A tile (+ xn to HBM, row statistics to smem), then dz -> A tile
-//   warp 4       MMA issuer (event loop over: H quarter, DA quarter, dh chunk; probes instead of blocking waits)
-//   warp 5       weight copies (three lanes, one per stream: W1 / W2 / W1t pieces continuously, 48 KB per quarter)
-//   warp 6       TMA stores of the a / dh chunks
-//   warps 8-15   activation (two groups, chunks round-robin; one warp per TMEM lane quarter in each)
-//   warps 16-23  LayerNorm-backward epilogue (two warps per lane quarter, 32 of the 64 channels each)
-constexpr int NT_BWD = 768;
-constexpr int W_PIECE = 64 * 128;                   // one 64-row x 32-float piece of a streamed weight image (8 KB)
-constexpr int NPIECE = 3;
-constexpr int SMEM_BWD = 1024 + 2 * XN_BYTES + 4 * CHUNK_BYTES + 3 * NPIECE * W_PIECE + 2 * BM * 8 + 2 * 2 * BM * 8 + 1536 + 512;
 
 struct FfnBwdArgs {
-    const float* x; long long ldx;
-    const float* dz; long long lddz;
-    const float* dout; long long lddo;
-    const float* res2; long long ldr2;
-    float* dx; long long lddx;
-    float* xn_out;
-    const float* ln_g; const float* ln_b; const float* b1;
-    const float* W1p; const float* W2tp; const float* W1tp;
-    float* dgamma; float* dbeta;
-    long long M;
-    unsigned long long seed1; unsigned int thr; float inv_keep;
-    const unsigned long long* seed_dev;
-    long long* dbg;
+    const float* x; long long ldx; const float* dz; long long lddz;
+    const float* ln_g; const float* ln_b; const float* W1p; const float* b1; const float* W2tp;
+    long long M; unsigned long long seed1; unsigned int thr; float inv_keep; const unsigned long long* seed_dev;
+    float* a_out; float* dh_out; float* xn_out; float* stats;
 };
 
-template <int N>
-__device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N>
-__device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-
-// TMA store of one K-major SWIZZLE_128B chunk (128 rows x 32 floats) to a row-major (M, 256) tensor; rows past M are clipped by the unit
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src_smem), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-
-__global__ void __launch_bounds__(NT_BWD, 1) ffn_bwd_kernel(const __grid_constant__ FfnBwdArgs g, const __grid_constant__ CUtensorMap tmA,
-                                                           const __grid_constant__ CUtensorMap tmDh) {
+__global__ void __launch_bounds__(NT, 1) ffn_bwd_kernel(const __grid_constant__ FfnBwdArgs g) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t sXn = base, sDz = sXn + XN_BYTES, sRingD = sDz + XN_BYTES, sRingA = sRingD + 2 * CHUNK_BYTES, sW2 = sRingA + 2 * CHUNK_BYTES;
-    const uint32_t sW1t = sW2 + NPIECE * W_PIECE, sW1 = sW1t + NPIECE * W_PIECE;
-    const uint32_t sStat = sW1 + NPIECE * W_PIECE;                 // float2 [2][128]: (mean, rstd) of the rows of the tile
-    const uint32_t sExch = sStat + 2 * BM * 8;                      // float2 [2 tiles][2 halves][128]: partial (sum g, sum g xhat) of a half row
-    const uint32_t sPar = sExch + 2 * 2 * BM * 8;                   // gamma[64] beta[64] b1[256]
-    float2* stat = reinterpret_cast<float2*>(base_ptr + (sStat - base));
-    float2* exch = reinterpret_cast<float2*>(base_ptr + (sExch - base));
-    float* par = reinterpret_cast<float*>(base_ptr + (sPar - base));
-    const uint32_t bars = sPar + 1536;
-    const uint32_t xn_full = bars, dz_full = bars + 8, xn_free = bars + 16, dz_free = bars + 24;
-    auto h_full = [&](int q) { return bars + 32u + 8u * q; };        // [4]
-    auto da_full = [&](int s) { return bars + 64u + 8u * s; };       // [2]
-    auto hid_full = [&](int s) { return bars + 80u + 8u * s; };      // [2]
-    auto hid_empty = [&](int s) { return bars + 96u + 8u * s; };     // [2]   two arrivals: tensor pipe done (commit) + TMA stores have read the slot
-    auto acc_full = [&](int b) { return bars + 112u + 8u * b; };     // [2]
-    auto acc_empty = [&](int b) { return bars + 128u + 8u * b; };    // [2]
-    auto w2_full = [&](int s) { return bars + 144u + 8u * s; };      // [3]
-    auto w2_empty = [&](int s) { return bars + 168u + 8u * s; };     // [3]
-    auto w1t_full = [&](int s) { return bars + 192u + 8u * s; };     // [3]
-    auto w1t_empty = [&](int s) { return bars + 216u + 8u * s; };    // [3]
-    auto w1_full = [&](int s) { return bars + 240u + 8u * s; };      // [3]
-    auto w1_empty = [&](int s) { return bars + 264u + 8u * s; };     // [3]
-    const uint32_t tmem_ptr_addr = bars + 288u;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ntiles = (int)((g.M + BM - 1) / BM);
-    const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int NQ = 4 * my_tiles;
-
-    if (tid == 0) {
-        mbar_init(xn_full, 4); mbar_init(dz_full, 4); mbar_init(xn_free, 1); mbar_init(dz_free, 1);
-        for (int q = 0; q < 4; ++q) mbar_init(h_full(q), 1);
-        for (int s = 0; s < 2; ++s) { mbar_init(da_full(s), 1); mbar_init(hid_full(s), 4); mbar_init(hid_empty(s), 2); mbar_init(acc_full(s), 1); mbar_init(acc_empty(s), 8); }
-        for (int s = 0; s < NPIECE; ++s) { mbar_init(w2_full(s), 1); mbar_init(w2_empty(s), 1); mbar_init(w1t_full(s), 1); mbar_init(w1t_empty(s), 1); mbar_init(w1_full(s), 1); mbar_init(w1_empty(s), 1); }
-        fence_barrier_init();
-    }
-    for (int i = tid; i < 384; i += NT_BWD) par[i] = i < 64 ? __ldg(g.ln_g + i) : i < 128 ? __ldg(g.ln_b + i - 64) : __ldg(g.b1 + i - 128);
-    if (warp == 4) tmem_alloc(tmem_ptr_addr, TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_addr));
-    const float* gam = par; const float* bet = par + 64; const float* b1s = par + 128;
-    // TMEM columns: H quarters [0, 256), DA slots [256, 384), dxn accumulators [384, 512)
-    constexpr uint32_t T_DA = 256, T_ACC = 384;
-
-    // register budget: 768 threads start with 80 each; the issue / copy warpgroup hands 24 x 128 back and the producers (64 row values in
-    // flight) take them.  Local-memory spills go to L2 here (the L1 carve-out is all shared memory), so every role is written to fit.
-    if (warp < 4) {
-        // ================================ row producers ================================
-        reg_inc<104>();
-        for (int lt = 0; lt < my_tiles; ++lt) {
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + tid;
-            const bool ok = row < g.M;
-            float v[64];
-            if (ok) {
-                const float4* xr = reinterpret_cast<const float4*>(g.x + row * g.ldx);
+    uint8_t* const bp = smem_raw + (base - smem_u32(smem_raw));
+    uint8_t* const sW1 = bp;                       // W1 image: 2 chunks x 256 rows (h = xn W1^T)
+    uint8_t* const sW2t = bp + W_BYTES;            // W2^T image: 2 chunks x 256 rows (dz W2)
+    uint8_t* const sXn = bp + 2 * W_BYTES;         // 2 chunks x 64 rows
+    uint8_t* const sDz = sXn + 2 * CHUNK;          // 2 chunks x 64 rows
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, fg = lane >> 2, ft = lane & 3;
+    const bool drop_on = g.thr != 0u;
+    const uint32_t thr16 = g.thr >> 16;
+    const uint32_t s1 = cmgan_seed32(cmgan_eff_seed(g.seed1, g.seed_dev));
+    copy_image(sW1, g.W1p, W_BYTES);
+    copy_image(sW2t, g.W2tp, W_BYTES);
+    const long ntiles = (g.M + BM - 1) / BM;
+    for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long m0 = tile * BM;
+        const float2 st = ln_tile(g.x, g.ldx, m0, g.M, g.ln_g, g.ln_b, sXn, g.xn_out);
+        {   // statistics for the LayerNorm backward; dz (already a tf32 operand) -> second A operand
+            const int r = threadIdx.x >> 1, half = threadIdx.x & 1;
+            const long m = m0 + r;
+            if (half == 0 && m < g.M) reinterpret_cast<float2*>(g.stats)[m] = st;
 #pragma unroll
-                for (int c4 = 0; c4 < 16; ++c4) { const float4 t = __ldg(xr + c4); v[4 * c4] = t.x; v[4 * c4 + 1] = t.y; v[4 * c4 + 2] = t.z; v[4 * c4 + 3] = t.w; }
-            } else {
-#pragma unroll
-                for (int k = 0; k < 64; ++k) v[k] = 0.f;
+            for (int q = 0; q < 8; ++q) {
+                const float4 t = m < g.M ? __ldg(reinterpret_cast<const float4*>(g.dz + m * g.lddz + half * 32 + 4 * q)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                *reinterpret_cast<float4*>(sDz + half * CHUNK + swz(r, 4 * q)) = t;
             }
-            float s = 0.f;
-#pragma unroll
-            for (int k = 0; k < 64; ++k) s += v[k];
-            const float mean = s * (1.f / 64.f);
-            float q = 0.f;
-#pragma unroll
-            for (int k = 0; k < 64; ++k) { const float d = v[k] - mean; q = fmaf(d, d, q); }
-            const float rstd = rsqrtf(q * (1.f / 64.f) + 1e-5f);
-#pragma unroll
-            for (int k = 0; k < 64; ++k) v[k] = to_tf32(fmaf((v[k] - mean) * rstd, gam[k], bet[k]));
-            if (ok) {
-                float4* xo = reinterpret_cast<float4*>(g.xn_out + row * C);
-#pragma unroll
-                for (int c4 = 0; c4 < 16; ++c4) xo[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-            }
-            if (lt >= 2) mbar_wait(acc_empty(lt & 1), (uint32_t)(((lt - 2) >> 1) & 1));     // the epilogue of tile lt - 2 has read its row statistics
-            stat[(lt & 1) * BM + tid] = make_float2(mean, rstd);
-            FFN_STAMP(4 * lt);
-            if (lt > 0) mbar_wait(xn_free, (uint32_t)((lt - 1) & 1));     // every H quarter of the previous tile has been issued
-            FFN_STAMP(4 * lt + 1);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) st_shared_v4(sXn + (uint32_t)(c >> 3) * CHUNK_BYTES + sw_off(tid, c & 7), v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(xn_full);
-            if (ok) {
-                const float4* zr = reinterpret_cast<const float4*>(g.dz + row * g.lddz);
-#pragma unroll
-                for (int c4 = 0; c4 < 16; ++c4) { const float4 t = __ldg(zr + c4); v[4 * c4] = t.x; v[4 * c4 + 1] = t.y; v[4 * c4 + 2] = t.z; v[4 * c4 + 3] = t.w; }
-            } else {
-#pragma unroll
-                for (int k = 0; k < 64; ++k) v[k] = 0.f;
-            }
-            FFN_STAMP(4 * lt + 2);
-            if (lt > 0) mbar_wait(dz_free, (uint32_t)((lt - 1) & 1));     // every DA quarter of the previous tile has been issued
-            FFN_STAMP(4 * lt + 3);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) st_shared_v4(sDz + (uint32_t)(c >> 3) * CHUNK_BYTES + sw_off(tid, c & 7), v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(dz_full);
         }
-    } else if (warp < 8) {
-        // ================================ MMA issuer + TMA stores (warp 4), weight copies (warp 5) ================================
-        reg_dec<56>();
-        if (warp == 4 && lane == 0 && my_tiles > 0) {
-            const uint32_t idesc64 = make_idesc_tf32(BM, 64, 0, 0);
-            int Gh = 0, Gd = 0;              // next H / DA quarter to issue (global quarter index = 4 tile + quarter)
-            long cj = 0;                     // next dh chunk to consume (8 per tile)
-            const long NC = 8L * my_tiles;
-            int xn_tile = -1, dz_tile = -1;  // tiles whose xn / dz have been seen in the A tile
-            uint32_t idle = 0;
-            while (cj < NC) {
-                bool progress = false;
-                const int cq = (int)(cj >> 1);                       // quarters completely consumed by the activation warps
-                // ---- H quarter: region q free once quarter Gh - 4 is consumed; xn of its tile must be in the A tile
-                if (Gh < NQ && (Gh < 4 || cq > Gh - 4)) {
-                    const int t = Gh >> 2, q = Gh & 3;
-                    if (xn_tile < t && mbar_test(xn_full, (uint32_t)(t & 1))) { xn_tile = t; tc_fence_after(); }
-                    const long p0 = 2L * Gh, p1 = p0 + 1;
-                    if (xn_tile >= t && mbar_test(w1_full((int)(p0 % NPIECE)), (uint32_t)((p0 / NPIECE) & 1)) &&
-                        mbar_test(w1_full((int)(p1 % NPIECE)), (uint32_t)((p1 / NPIECE) & 1))) {
-                        tc_fence_after();
+        fence_proxy_async();
+        __syncthreads();
+#pragma unroll 1
+        for (int qt = 0; qt < 4; ++qt) {            // hidden columns 64 qt .. 64 qt + 63
+            float acc[4][8], dacc[4][8];
+            const uint32_t wrow = (uint32_t)qt * 64 * 128;
+            wgmma_fence();
+            mma_chunk<4, 4>(acc, gmma_desc_sw128(base + 2 * W_BYTES), gmma_desc_sw128(base + wrow), true);
+            mma_chunk<4, 4>(acc, gmma_desc_sw128(base + 2 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128 + wrow), false);
+            mma_chunk<4, 4>(dacc, gmma_desc_sw128(base + 2 * W_BYTES + 2 * CHUNK), gmma_desc_sw128(base + W_BYTES + wrow), true);
+            mma_chunk<4, 4>(dacc, gmma_desc_sw128(base + 2 * W_BYTES + 3 * CHUNK), gmma_desc_sw128(base + W_BYTES + 256 * 128 + wrow), false);
+            wgmma_commit();
+            wgmma_wait<0>();
 #pragma unroll
-                        for (int kc = 0; kc < 2; ++kc) {
-                            const long p = p0 + kc;
-                            const uint64_t adesc = make_desc_sw128(sXn + kc * CHUNK_BYTES, 16, 1024);
-                            const uint64_t bdesc = make_desc_sw128(sW1 + (uint32_t)(p % NPIECE) * W_PIECE, 16, 1024);
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
-                            for (int k = 0; k < 4; ++k)
-                                umma_tf32(tmem_base + (uint32_t)(q * 64), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc64, (kc | k) != 0 ? 1u : 0u);
-                            umma_commit(w1_empty((int)(p % NPIECE)));
-                        }
-                        umma_commit(h_full(q));
-                        if (q == 3) umma_commit(xn_free);            // xn of tile t consumed: the producers may write the next tile's
-                        ++Gh; progress = true;
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const long m = m0 + 16 * warp + fg + 8 * hh;
+                        if (m >= g.M) continue;
+                        const int n = 64 * qt + 16 * j + 8 * i + 2 * ft;
+                        const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b1 + n));
+                        const float2 ds = drop_pair(m, n, HID, s1, thr16, g.inv_keep, drop_on);
+                        const float h0 = acc[j][4 * i + 2 * hh] + bb.x, h1 = acc[j][4 * i + 2 * hh + 1] + bb.y;
+                        *reinterpret_cast<float2*>(g.a_out + m * HID + n) = make_float2(to_tf32(swishf_(h0) * ds.x), to_tf32(swishf_(h1) * ds.y));
+                        *reinterpret_cast<float2*>(g.dh_out + m * HID + n) =
+                            make_float2(to_tf32(dacc[j][4 * i + 2 * hh] * dswishf_(h0) * ds.x), to_tf32(dacc[j][4 * i + 2 * hh + 1] * dswishf_(h1) * ds.y));
                     }
-                }
-                // ---- DA quarter: slot Gd % 2 free once quarter Gd - 2 is consumed; dz of its tile in the A tile; both W2 pieces landed
-                if (Gd < NQ && (Gd < 2 || cq > Gd - 2)) {
-                    const int t = Gd >> 2, q = Gd & 3;
-                    if (dz_tile < t && mbar_test(dz_full, (uint32_t)(t & 1))) { dz_tile = t; tc_fence_after(); }
-                    const long p0 = 2L * Gd, p1 = p0 + 1;
-                    if (dz_tile >= t && mbar_test(w2_full((int)(p0 % NPIECE)), (uint32_t)((p0 / NPIECE) & 1)) &&
-                        mbar_test(w2_full((int)(p1 % NPIECE)), (uint32_t)((p1 / NPIECE) & 1))) {
-                        tc_fence_after();
-#pragma unroll
-                        for (int kc = 0; kc < 2; ++kc) {
-                            const long p = p0 + kc;
-                            const uint64_t adesc = make_desc_sw128(sDz + kc * CHUNK_BYTES, 16, 1024);
-                            const uint64_t bdesc = make_desc_sw128(sW2 + (uint32_t)(p % NPIECE) * W_PIECE, 16, 1024);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)
-                                umma_tf32(tmem_base + T_DA + (uint32_t)((Gd & 1) * 64), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc64, (kc | k) != 0 ? 1u : 0u);
-                            umma_commit(w2_empty((int)(p % NPIECE)));
-                        }
-                        umma_commit(da_full(Gd & 1));
-                        if (q == 3) umma_commit(dz_free);
-                        ++Gd; progress = true;
-                    }
-                }
-                // ---- a / dh chunk: dh -> dxn accumulator; both chunks -> HBM by TMA
-                {
-                    const int lt = (int)(cj >> 3), j = (int)(cj & 7), buf = lt & 1, sl = (int)(cj & 1);
-                    bool ready = mbar_test(hid_full(sl), (uint32_t)((cj >> 1) & 1)) && mbar_test(w1t_full((int)(cj % NPIECE)), (uint32_t)((cj / NPIECE) & 1));
-                    if (ready && j == 0) ready = mbar_test(acc_empty(buf), (uint32_t)(((lt >> 1) & 1) ^ 1));
-                    if (ready) {
-                        FFN_STAMP((int)cj);
-                        tc_fence_after();
-                        const uint64_t adesc = make_desc_sw128(sRingD + sl * CHUNK_BYTES, 16, 1024);
-                        const uint64_t bdesc = make_desc_sw128(sW1t + (uint32_t)(cj % NPIECE) * W_PIECE, 16, 1024);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_tf32(tmem_base + T_ACC + (uint32_t)(buf * 64), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc64, (j | k) != 0 ? 1u : 0u);
-                        umma_commit(hid_empty(sl));                  // 1st of the slot's two releases
-                        umma_commit(w1t_empty((int)(cj % NPIECE)));
-                        if (j == 7) umma_commit(acc_full(buf));
-                        ++cj; progress = true;
-                    }
-                }
-                if (progress) idle = 0;
-                else if (++idle > (1u << 27)) __trap();           // protocol bug: fail loudly instead of hanging the device
-            }
-        } else if (warp == 5 && lane < 3 && my_tiles > 0) {
-            // three independent streams of 8 KB pieces, one lane each (a blocked stream must not hold the other two back):
-            // lane 0: H weight (piece p = 2 G + kc), lane 1: DA weight (same indexing), lane 2: dxn weight (piece = chunk index, K chunk 2 q + c2)
-            const long NP = 2L * NQ;
-            for (long p = 0; p < NP; ++p) {
-                const int sl = (int)(p % NPIECE), q = (int)((p >> 1) & 3), kc = (int)(p & 1);
-                const uint32_t par = (uint32_t)(((p / NPIECE) & 1) ^ 1);
-                if (lane == 0) {
-                    mbar_wait(w1_empty(sl), par);
-                    mbar_arrive_expect_tx(w1_full(sl), (uint32_t)W_PIECE);
-                    bulk_g2s(sW1 + sl * W_PIECE, g.W1p + ((long)kc * (HID * 128) + (long)q * W_PIECE) / 4, (uint32_t)W_PIECE, w1_full(sl));
-                } else if (lane == 1) {
-                    mbar_wait(w2_empty(sl), par);
-                    mbar_arrive_expect_tx(w2_full(sl), (uint32_t)W_PIECE);
-                    bulk_g2s(sW2 + sl * W_PIECE, g.W2tp + ((long)kc * (HID * 128) + (long)q * W_PIECE) / 4, (uint32_t)W_PIECE, w2_full(sl));
-                } else {
-                    mbar_wait(w1t_empty(sl), par);
-                    mbar_arrive_expect_tx(w1t_full(sl), (uint32_t)W_PIECE);
-                    bulk_g2s(sW1t + sl * W_PIECE, g.W1tp + ((long)(2 * q + kc) * W_PIECE) / 4, (uint32_t)W_PIECE, w1t_full(sl));
-                }
-            }
-        } else if (warp == 6 && lane == 0 && my_tiles > 0) {
-            // a / dh chunks -> HBM by TMA, in ring order; the slot's 2nd release once the unit has read it (the issuer never waits on this)
-            const long NC = 8L * my_tiles;
-            for (long cj = 0; cj < NC; ++cj) {
-                const int lt = (int)(cj >> 3), j = (int)(cj & 7), sl = (int)(cj & 1);
-                mbar_wait(hid_full(sl), (uint32_t)((cj >> 1) & 1));
-                const int row0 = (int)(((long)blockIdx.x + (long)lt * gridDim.x) * BM);
-                tma_store_2d(&tmDh, sRingD + sl * CHUNK_BYTES, j * 32, row0);
-                tma_store_2d(&tmA, sRingA + sl * CHUNK_BYTES, j * 32, row0);
-                bulk_commit();
-                bulk_wait_read<0>();
-                mbar_arrive(hid_empty(sl));
-            }
-            bulk_wait_all<0>();                                      // every a / dh store has landed before the CTA retires
         }
-        __syncwarp();
-    } else if (warp < 16) {
-        // ================================ activation (warps 8-15) ================================
-        // group (warp - 8) / 4 takes the chunks of its parity: both groups work on the two halves of the same quarter
-        const int lq = warp & 3, grp = (warp - 8) >> 2, rloc = lq * 32 + lane;
-        const uint32_t seed1_32 = cmgan_seed32(cmgan_eff_seed(g.seed1, g.seed_dev));
-        const uint32_t thr16 = g.thr >> 16;
-        const bool drop_on = g.thr != 0u;
-        const long NC = 8L * my_tiles;
-        const uint32_t dstD = sRingD + grp * CHUNK_BYTES, dstA = sRingA + grp * CHUNK_BYTES;
-        for (long cj = grp; cj < NC; cj += 2) {
-            const int lt = (int)(cj >> 3), j = (int)(cj & 7), q = j >> 1;
-            const long G = cj >> 1;
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + rloc;
-            FFN_STAMP(3 * (int)(cj >> 1));
-            mbar_wait(h_full(q), (uint32_t)(lt & 1));
-            mbar_wait(da_full((int)(G & 1)), (uint32_t)((G >> 1) & 1));
-            tc_fence_after();
-            FFN_STAMP(3 * (int)(cj >> 1) + 1);
-#pragma unroll
-            for (int hf = 0; hf < 2; ++hf) {                         // 16 hidden columns at a time (register budget)
-                const int n0 = j * 32 + hf * 16;
-                uint32_t rh[16], rd[16];
-                tmem_ld16_nowait(tmem_base + (uint32_t)n0 + ((uint32_t)(lq * 32) << 16), rh);
-                tmem_ld16_nowait(tmem_base + T_DA + (uint32_t)((G & 1) * 64 + grp * 32 + hf * 16) + ((uint32_t)(lq * 32) << 16), rd);
-                tmem_wait_ld();
-                const uint32_t pair0 = (uint32_t)(((unsigned long long)row * HID + (unsigned long long)n0) >> 1);
-                if (hf == 0) mbar_wait(hid_empty(grp), (uint32_t)(((cj >> 1) & 1) ^ 1));      // tensor pipe and TMA have read the previous occupants
-#pragma unroll
-                for (int o8 = 0; o8 < 2; ++o8) {                     // 8 columns at a time from registers to the rings: no spill (L1 is all shared memory)
-                    float av[8], dv[8];
-#pragma unroll
-                    for (int p = 0; p < 4; ++p) {
-                        const int e = 8 * o8 + 2 * p;
-                        float d0 = 1.f, d1 = 1.f;
-                        if (drop_on) {
-                            const uint32_t h = cmgan_mix32(((pair0 + (uint32_t)(4 * o8 + p)) * 0x9E3779B1u) ^ seed1_32);
-                            d0 = (h & 0xFFFFu) >= thr16 ? g.inv_keep : 0.f; d1 = (h >> 16) >= thr16 ? g.inv_keep : 0.f;
-                        }
-                        const float h0 = __uint_as_float(rh[e]) + b1s[n0 + e], h1 = __uint_as_float(rh[e + 1]) + b1s[n0 + e + 1];
-                        const float s0 = sigmoidf_(h0), s1 = sigmoidf_(h1);
-                        av[2 * p] = to_tf32(h0 * s0 * d0);
-                        av[2 * p + 1] = to_tf32(h1 * s1 * d1);
-                        dv[2 * p] = to_tf32(__uint_as_float(rd[e]) * d0 * (s0 * (1.f + h0 * (1.f - s0))));
-                        dv[2 * p + 1] = to_tf32(__uint_as_float(rd[e + 1]) * d1 * (s1 * (1.f + h1 * (1.f - s1))));
-                    }
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        st_shared_v4(dstD + sw_off(rloc, hf * 4 + o8 * 2 + c), dv[4 * c], dv[4 * c + 1], dv[4 * c + 2], dv[4 * c + 3]);
-                        st_shared_v4(dstA + sw_off(rloc, hf * 4 + o8 * 2 + c), av[4 * c], av[4 * c + 1], av[4 * c + 2], av[4 * c + 3]);
-                    }
-                }
-            }
-            fence_proxy_async();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(hid_full(grp));
-            FFN_STAMP(3 * (int)(cj >> 1) + 2);
-        }
-    } else {
-        // ================================ LayerNorm-backward epilogue (warps 16-23) ================================
-        // thread = half a row (32 channels), swept twice in pieces of 16 channels: dxn is simply re-read from TMEM and x from L2 (the warps
-        // have time to spare), so only 3 x 16 values are live.  The two halves of a row exchange their partial sums (sum g, sum g xhat)
-        // through shared memory around a 64-thread named barrier.
-        const int ew = warp - 16, lq = warp & 3, hv = ew >> 2, rloc = lq * 32 + lane;
-        float accg = 0.f, accb = 0.f;                           // dgamma / dbeta share of this lane (channel: see the end of the loop)
-        auto reduce16 = [&](float v[16]) {                      // column sums over the warp's 32 rows: afterwards v[0] = total of entry lane >> 1
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const bool up = lane & 16;
-                const float send = up ? v[i] : v[i + 8], keep = up ? v[i + 8] : v[i];
-                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const bool up = lane & 8;
-                const float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i];
-                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const bool up = lane & 4;
-                const float send = up ? v[i] : v[i + 2], keep = up ? v[i + 2] : v[i];
-                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-            }
-            {
-                const bool up = lane & 2;
-                const float send = up ? v[0] : v[1], keep = up ? v[1] : v[0];
-                v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-            }
-            v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-        };
-        for (int lt = 0; lt < my_tiles; ++lt) {
-            const int buf = lt & 1;
-            const long row = ((long)blockIdx.x + (long)lt * gridDim.x) * BM + rloc;
-            const bool ok = row < g.M;
-            const float4* xr = reinterpret_cast<const float4*>(g.x + (ok ? row : 0) * g.ldx) + hv * 8;
-            float4 xv[8];                                        // first sweep's x: requested before the accumulator is ready
-#pragma unroll
-            for (int c4 = 0; c4 < 8; ++c4) xv[c4] = ok ? __ldg(xr + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            FFN_STAMP(3 * lt);
-            mbar_wait(acc_full(buf), (uint32_t)((lt >> 1) & 1));
-            FFN_STAMP(3 * lt + 1);
-            tc_fence_after();
-            const float2 st = stat[(lt & 1) * BM + rloc];
-            const uint32_t taddr = tmem_base + T_ACC + (uint32_t)(buf * 64 + hv * 32) + ((uint32_t)(lq * 32) << 16);
-            float c1 = 0.f, c2 = 0.f;
-#pragma unroll
-            for (int pc = 0; pc < 2; ++pc) {
-                float r[16];
-                tmem_ld16f_nowait(taddr + pc * 16, r);
-                tmem_wait_ld();
-#pragma unroll
-                for (int c4 = 0; c4 < 4; ++c4) {
-                    const float4 t = xv[pc * 4 + c4];
-                    const float xs[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float gk = r[4 * c4 + j] * gam[32 * hv + 16 * pc + 4 * c4 + j];
-                        c1 += gk; c2 = fmaf(gk, (xs[j] - st.x) * st.y, c2);
-                    }
-                }
-            }
-            if (!ok) { c1 = 0.f; c2 = 0.f; }
-            exch[((lt & 1) * 2 + hv) * BM + rloc] = make_float2(c1, c2);
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + lq) : "memory");          // the two warps that share these 32 rows
-            const float2 oth = exch[((lt & 1) * 2 + (hv ^ 1)) * BM + rloc];
-            c1 = (c1 + oth.x) * (1.f / 64.f); c2 = (c2 + oth.y) * (1.f / 64.f);
-#pragma unroll
-            for (int pc = 0; pc < 2; ++pc) {
-                float r[16], xh[16];
-                tmem_ld16f_nowait(taddr + pc * 16, r);
-#pragma unroll
-                for (int c4 = 0; c4 < 4; ++c4) {
-                    const float4 t = ok ? __ldg(xr + pc * 4 + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    xh[4 * c4] = (t.x - st.x) * st.y; xh[4 * c4 + 1] = (t.y - st.x) * st.y; xh[4 * c4 + 2] = (t.z - st.x) * st.y; xh[4 * c4 + 3] = (t.w - st.x) * st.y;
-                }
-                tmem_wait_ld();
-                if (pc == 1) {                                       // last read of this accumulator (and of the tile's row statistics)
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(acc_empty(buf));
-                }
-                if (ok) {
-                    const float4* dor = reinterpret_cast<const float4*>(g.dout + row * g.lddo) + hv * 8 + pc * 4;
-                    const float4* r2 = g.res2 ? reinterpret_cast<const float4*>(g.res2 + row * g.ldr2) + hv * 8 + pc * 4 : nullptr;
-                    float4* dxr = reinterpret_cast<float4*>(g.dx + row * g.lddx) + hv * 8 + pc * 4;
-#pragma unroll
-                    for (int c4 = 0; c4 < 4; ++c4) {
-                        float4 o = __ldg(dor + c4);
-                        if (r2) { const float4 e = __ldg(r2 + c4); o.x += e.x; o.y += e.y; o.z += e.z; o.w += e.w; }
-                        const int k = 4 * c4, kg = 32 * hv + 16 * pc + k;
-                        o.x += st.y * (r[k + 0] * gam[kg + 0] - c1 - xh[k + 0] * c2);
-                        o.y += st.y * (r[k + 1] * gam[kg + 1] - c1 - xh[k + 1] * c2);
-                        o.z += st.y * (r[k + 2] * gam[kg + 2] - c1 - xh[k + 2] * c2);
-                        o.w += st.y * (r[k + 3] * gam[kg + 3] - c1 - xh[k + 3] * c2);
-                        dxr[c4] = o;
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < 16; ++k) { r[k] = ok ? r[k] : 0.f; xh[k] *= r[k]; }
-                reduce16(xh);                                        // dgamma: column sums of dxn * xhat
-                reduce16(r);                                         // dbeta:  column sums of dxn
-                // every lane pair (2 c, 2 c + 1) now holds the totals of channel 32 hv + 16 pc + c: the even lane keeps piece 0's, the odd lane piece 1's
-                if ((lane & 1) == pc) { accg += xh[0]; accb += r[0]; }
-            }
-            FFN_STAMP(3 * lt + 2);
-        }
-        if (my_tiles > 0) {
-            const int ch = 32 * hv + 16 * (lane & 1) + (lane >> 1);
-            atomicAdd(g.dgamma + ch, accg);
-            atomicAdd(g.dbeta + ch, accb);
-        }
-    }
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
+        __syncthreads();          // sXn / sDz are rewritten by the next tile
     }
 }
 
-long long* g_ffn_dbg = nullptr;
-
-using PFN_encodeTiled_ffn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                          const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled_ffn get_encoder_ffn() {
-    static PFN_encodeTiled_ffn encode = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            encode = reinterpret_cast<PFN_encodeTiled_ffn>(fn);
+template <typename K>
+int prepare(K kernel, size_t smem, const char* name) {
+    static bool set = false;
+    if (!set) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { cmgan_set_error("%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e)); return -1; }
+        set = true;
     }
-    return encode;
-}
-int g_sms = 0;
-int num_sms() {
-    if (g_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    return g_sms;
+    return 0;
 }
 
 }  // namespace
 
-// developer aid: a device buffer of 32 warps x 64 clock64 stamps filled by CTA 0 of the next cmgan_ffn_fwd launches (nullptr switches it off)
-CMGAN_API int cmgan_ffn_debug_timeline(long long* buf) { g_ffn_dbg = buf; return 0; }
-
-// out = x + alpha * drop(seed2)( W2 ( swish(W1 LN(x) + b1) * drop(seed1) ) + b2 ).  W1p / W2p: the weights re-tiled by cmgan_pack_weights
-// (W1 (256, 64): sb_k = 1, sb_n = 64, N = 256, Cin = 64;  W2 (64, 256): sb_k = 1, sb_n = 256, N = 64, Cin = 256).  thr = p * 2^32 (0: no dropout).
-// Dropout element indices are row * 256 + n (hidden) and row * 64 + c (output), i.e. the masks cmgan_dropout_mask exports for those seeds.
+// out = x + alpha * drop2(W2 (swish(W1 LN(x) + b1) * drop1) + b2); W1p / W2p: cmgan_pack_weight images of W1 (256 x 64) and W2 (64 x 256)
 CMGAN_API int cmgan_ffn_fwd(const float* x, long long ldx, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1,
                             const float* W2p, const float* b2, float alpha, unsigned long long seed1, unsigned long long seed2, unsigned int thr,
                             float inv_keep, const unsigned long long* seed_dev, float* out, long long ldo, void* stream) {
-    CMGAN_REQUIRE(x && out && ln_g && ln_b && W1p && b1 && W2p && b2, "cmgan_ffn_fwd: null pointer");
-    CMGAN_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && (((uintptr_t)x | (uintptr_t)out) & 15) == 0, "cmgan_ffn_fwd: rows must be 16-byte aligned");
-    CMGAN_REQUIRE((((uintptr_t)W1p | (uintptr_t)W2p) & 127) == 0, "cmgan_ffn_fwd: weight images must be 128-byte aligned");
+    CMGAN_REQUIRE(x && out && ln_g && ln_b && W1p && b1 && W2p && b2 && M >= 0 && ldx % 4 == 0 && ldo % 2 == 0, "cmgan_ffn_fwd: bad arguments");
     if (M == 0) return 0;
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(ffn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_FWD);
-        if (e != cudaSuccess) { cmgan_set_error("cmgan_ffn_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
-        attr_set = true;
-    }
-    FfnFwdArgs a;
-    a.x = x; a.ldx = ldx; a.out = out; a.ldo = ldo; a.ln_g = ln_g; a.ln_b = ln_b; a.W1p = W1p; a.b1 = b1; a.W2p = W2p; a.b2 = b2; a.M = M; a.alpha = alpha;
-    a.seed1 = seed1; a.seed2 = seed2; a.thr = thr; a.inv_keep = inv_keep; a.seed_dev = seed_dev;
-    a.dbg = g_ffn_dbg;
-    const int ntiles = (int)((M + BM - 1) / BM);
-    const int grid = ntiles < num_sms() ? ntiles : num_sms();
-    ffn_fwd_kernel<<<grid, NTHREADS, SMEM_FWD, (cudaStream_t)stream>>>(a);
+    const size_t smem = 1024 + 2 * W_BYTES + 2 * CHUNK + 8 * CHUNK;
+    if (prepare(ffn_fwd_kernel, smem, "ffn_fwd_kernel")) return -1;
+    FfnFwdArgs a{x, ldx, out, ldo, ln_g, ln_b, W1p, b1, W2p, b2, M, alpha, seed1, seed2, thr, inv_keep, seed_dev};
+    const long ntiles = (M + BM - 1) / BM;
+    const int grid = (int)(ntiles < cmgan_num_sms() ? ntiles : cmgan_num_sms());
+    ffn_fwd_kernel<<<grid, NT, smem, (cudaStream_t)stream>>>(a);
     return cmgan_check_launch("ffn_fwd_kernel");
 }
 
-// Data gradients of the same module (see ffn_bwd_kernel): dx = LNbwd((dz W2 (.) act'(h)) W1) + dout (+ res2), dgamma / dbeta accumulated, and
-// the operands of the two weight-gradient GEMMs written out: a = swish(h) * drop (M, 256), dh (M, 256), xn = LN(x) (M, 64).
-// Weight images (cmgan_pack_weights): W1p as in cmgan_ffn_fwd; W2tp = W2 (64, 256) with sb_k = 256, sb_n = 1, N = 256, Cin = 64;
-// W1tp = W1 (256, 64) with sb_k = 64, sb_n = 1, N = 64, Cin = 256.
+// Data gradients of the feed-forward from its input x and dz = alpha * drop2-mask * dout (a tf32 operand): dx = LN-backward(dh W1) + dout
+// (+ res2), dgamma / dbeta accumulated; leaves the weight-gradient operands a = swish(h) * drop1, dh and xn.  W1p: image of W1,
+// W2tp: image of W2 read transposed (256 x 64), W1tp: image of W1 read transposed (64 x 256).  ws: M * 66 floats of scratch.
 CMGAN_API int cmgan_ffn_bwd(const float* x, long long ldx, const float* dz, long long lddz, const float* dout, long long lddo, const float* res2,
                             long long ldr2, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1, const float* W2tp,
                             const float* W1tp, unsigned long long seed1, unsigned int thr, float inv_keep, const unsigned long long* seed_dev,
-                            float* dx, long long lddx, float* a_out, float* dh_out, float* xn_out, float* dgamma, float* dbeta, void* stream) {
-    CMGAN_REQUIRE(x && dz && dout && dx && a_out && dh_out && xn_out && ln_g && ln_b && W1p && b1 && W2tp && W1tp && dgamma && dbeta, "cmgan_ffn_bwd: null pointer");
-    CMGAN_REQUIRE(ldx % 4 == 0 && lddz % 4 == 0 && lddo % 4 == 0 && ldr2 % 4 == 0 && lddx % 4 == 0, "cmgan_ffn_bwd: leading dimensions must be multiples of 4");
-    CMGAN_REQUIRE((((uintptr_t)x | (uintptr_t)dz | (uintptr_t)dout | (uintptr_t)res2 | (uintptr_t)dx | (uintptr_t)a_out | (uintptr_t)dh_out | (uintptr_t)xn_out) & 15) == 0,
-                  "cmgan_ffn_bwd: rows must be 16-byte aligned");
-    CMGAN_REQUIRE((((uintptr_t)W1p | (uintptr_t)W2tp | (uintptr_t)W1tp) & 127) == 0, "cmgan_ffn_bwd: weight images must be 128-byte aligned");
-    CMGAN_REQUIRE(M < (1ll << 31), "cmgan_ffn_bwd: too many rows");
+                            float* dx, long long lddx, float* a_out, float* dh_out, float* xn_out, float* dgamma, float* dbeta, float* ws,
+                            void* stream) {
+    CMGAN_REQUIRE(x && dz && dout && ln_g && ln_b && W1p && b1 && W2tp && W1tp && dx && a_out && dh_out && xn_out && dgamma && dbeta && ws && M >= 0 &&
+                  ldx % 4 == 0 && lddz % 4 == 0, "cmgan_ffn_bwd: bad arguments");
     if (M == 0) return 0;
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(ffn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BWD);
-        if (e != cudaSuccess) { cmgan_set_error("cmgan_ffn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
-        attr_set = true;
-    }
-    // a / dh leave the kernel through TMA: (M, 256) row-major tensors, boxes of 128 rows x 32 floats in the SWIZZLE_128B shared-memory layout
-    PFN_encodeTiled_ffn encode = get_encoder_ffn();
-    CMGAN_REQUIRE(encode != nullptr, "cmgan_ffn_bwd: cuTensorMapEncodeTiled is not available from this driver");
-    alignas(64) CUtensorMap tmA, tmDh;
-    const cuuint64_t gdim[2] = {(cuuint64_t)HID, (cuuint64_t)M};
-    const cuuint64_t gstride[1] = {(cuuint64_t)HID * sizeof(float)};
-    const cuuint32_t box[2] = {32, (cuuint32_t)BM};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r1 = encode(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, a_out, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CUresult r2 = encode(&tmDh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dh_out, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CMGAN_REQUIRE(r1 == CUDA_SUCCESS && r2 == CUDA_SUCCESS, "cmgan_ffn_bwd: cuTensorMapEncodeTiled failed (%d, %d)", (int)r1, (int)r2);
-    FfnBwdArgs a;
-    a.x = x; a.ldx = ldx; a.dz = dz; a.lddz = lddz; a.dout = dout; a.lddo = lddo; a.res2 = res2; a.ldr2 = ldr2; a.dx = dx; a.lddx = lddx;
-    a.xn_out = xn_out; a.ln_g = ln_g; a.ln_b = ln_b; a.b1 = b1; a.W1p = W1p; a.W2tp = W2tp; a.W1tp = W1tp;
-    a.dgamma = dgamma; a.dbeta = dbeta; a.M = M; a.seed1 = seed1; a.thr = thr; a.inv_keep = inv_keep; a.seed_dev = seed_dev;
-    a.dbg = g_ffn_dbg;
-    const int ntiles = (int)((M + BM - 1) / BM);
-    const int grid = ntiles < num_sms() ? ntiles : num_sms();
-    ffn_bwd_kernel<<<grid, NT_BWD, SMEM_BWD, (cudaStream_t)stream>>>(a, tmA, tmDh);
-    return cmgan_check_launch("ffn_bwd_kernel");
+    const size_t smem = 1024 + 2 * W_BYTES + 4 * CHUNK;
+    if (prepare(ffn_bwd_kernel, smem, "ffn_bwd_kernel")) return -1;
+    float* dln = ws;                 // M x 64 (16-byte aligned rows for the row GEMM)
+    float* stats = ws + C * M;       // M x (mean, rstd)
+    FfnBwdArgs a{x, ldx, dz, lddz, ln_g, ln_b, W1p, b1, W2tp, M, seed1, thr, inv_keep, seed_dev, a_out, dh_out, xn_out, stats};
+    const long ntiles = (M + BM - 1) / BM;
+    const int grid = (int)(ntiles < cmgan_num_sms() ? ntiles : cmgan_num_sms());
+    ffn_bwd_kernel<<<grid, NT, smem, (cudaStream_t)stream>>>(a);
+    if (cmgan_check_launch("ffn_bwd_kernel")) return -1;
+    // dLN = dh W1 on the tensor-core row GEMM (W1 image read transposed, already packed)
+    CmganGemmArgs gm;
+    memset(&gm, 0, sizeof(gm));
+    gm.A = dh_out; gm.lda = HID; gm.B = W1tp; gm.sb_k = C; gm.sb_n = 1; gm.C = dln; gm.ldc = C;
+    gm.M = (int)M; gm.N = C; gm.Cin = HID; gm.ntaps = 1; gm.mul_y = gm.mul_x = gm.div_y = gm.div_x = 1;
+    gm.epi = CMGAN_EPI_NONE; gm.pro = CMGAN_PRO_NONE; gm.alpha = 1.f; gm.precision = 1;
+    gm.ws = const_cast<float*>(W1tp); gm.ws_floats = (long long)C * HID; gm.b_packed = 1;
+    const int rc = cmgan_gemm_rows_tc_launch(&gm, (cudaStream_t)stream);
+    CMGAN_REQUIRE(rc <= 0, "cmgan_ffn_bwd: dLN shape not covered by the tensor-core GEMM");
+    if (rc) return -1;
+    return cmgan_ln_bwd(dln, C, x, ldx, stats, ln_g, M, dout, lddo, res2, res2 ? ldr2 : 0, dx, lddx, dgamma, dbeta, stream);
 }

@@ -52,7 +52,7 @@ typedef struct CmganGemmArgs {
     unsigned long long pro_seed; unsigned int pro_thr; float pro_inv_keep;       // prologue dropout
     // wgrad only: D = upstream gradient rows (M x N), prod: 0 none, 1 = alpha * drop(m*N+n); dbias may be null
     const float* D; long long ldd; int prod; float* dbias;
-    int precision;             // 0 = fp32 FFMA, 1 = tf32 tcgen05 tensor cores (shapes the tensor path does not cover fall back to fp32 FFMA)
+    int precision;             // 0 = fp32 FFMA, 1 = tf32 wgmma tensor cores (shapes the tensor path does not cover fall back to fp32 FFMA)
     float* ws; long long ws_floats;   // tf32 path: scratch for the re-tiled weight operand, >= N_pad * Cin * ntaps floats (caller-owned)
     float* C2; long long ldc2;        // second output of CMGAN_EPI_SWISH_DUAL
     const unsigned long long* seed_dev;   // optional device counter added to both dropout seeds (CUDA-graph replays draw fresh masks)

@@ -1,4 +1,4 @@
-// Device helpers shared by the FFMA (gemm_simt.cu) and tcgen05 (gemm_tc.cu) implementations of the GEMM contract
+// Device helpers shared by the FFMA (gemm_simt.cu) and wgmma (gemm_tc.cu) implementations of the GEMM contract
 // in gemm_args.h: row decoding / implicit-convolution gather, A-operand prologues, epilogues.
 #pragma once
 #include "common.cuh"

@@ -1,6 +1,6 @@
 // fp32 FFMA GEMMs with fused gather (implicit convolution), A-operand prologues and epilogues.
 // These are the exact-fp32 baseline for every dense contraction of the path (see gemm_args.h for the
-// contract); the tf32 tcgen05 kernels in gemm_tc.cu implement the same contract for the hot shapes.
+// contract); the tf32 wgmma kernels in gemm_tc.cu / gemm_wgrad_tc.cu implement the same contract for the hot shapes.
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
 #include "gemm_args.h"
@@ -308,7 +308,7 @@ CMGAN_API int cmgan_gemm_rows_f32(const CmganGemmArgs* a, void* stream) {
     CMGAN_REQUIRE(a->B != nullptr, "cmgan_gemm_rows_f32: null B");
     if (a->M == 0) return 0;
     if (a->epi == CMGAN_EPI_DSWISH_DROP || a->epi == CMGAN_EPI_DBNSWISH) CMGAN_REQUIRE(a->aux != nullptr, "gemm_rows: epilogue needs aux");
-    if (a->precision == 1) {                       // tf32 tcgen05 path (gemm_tc.cu); 1 = shape not covered -> exact fp32 path below
+    if (a->precision == 1) {                       // tf32 wgmma path (gemm_tc.cu); 1 = shape not covered -> exact fp32 path below
         int rc = cmgan_gemm_rows_tc_launch(a, (cudaStream_t)stream);
         if (rc <= 0) return rc;
     }
@@ -337,12 +337,12 @@ CMGAN_API int cmgan_gemm_wgrad_f32(const CmganGemmArgs* a, void* stream) {
     if (validate(a, "cmgan_gemm_wgrad_f32")) return -1;
     CMGAN_REQUIRE(a->D != nullptr, "cmgan_gemm_wgrad_f32: null D");
     if (a->M == 0) return 0;
-    if (a->precision == 1) {                       // tf32 tcgen05 path (gemm_wgrad_tc.cu); 1 = shape not covered -> exact fp32 path below
+    if (a->precision == 1) {                       // tf32 wgmma path (gemm_wgrad_tc.cu); 1 = shape not covered -> exact fp32 path below
         int rc = cmgan_gemm_wgrad_tc_launch(a, (cudaStream_t)stream);
         if (rc <= 0) return rc;
     }
     if (a->ntaps * a->Cin <= NW_K && a->N <= NW_N && a->Cin < 16 && a->pro == CMGAN_PRO_NONE && a->prod == 0 && a->dbias == nullptr) {
-        long mch = cdiv(a->M, 148L * 4);
+        long mch = cdiv(a->M, (long)cmgan_num_sms() * 4);
         mch = cdiv(mch < 256 ? 256 : mch, NW_R) * NW_R;
         gemm_wgrad_narrow_kernel<<<(unsigned)cdiv(a->M, mch), NT, 0, (cudaStream_t)stream>>>(*a, (int)mch);
         return cmgan_check_launch("gemm_wgrad_narrow_kernel");

@@ -1,25 +1,22 @@
-// tf32 tensor-core implementation of the row-parallel GEMM contract (gemm_args.h) for sm_100a.
-// Persistent, warp-specialised: each CTA loops over 128-row output tiles; the accumulator lives in TMEM and is double-buffered so
-// that the epilogue of tile i overlaps the loads and MMAs of tile i+1.  Two shapes: 2 CTAs/SM x 10 warps (4 epilogue warps) for
-// narrow N, 1 CTA/SM x 14 warps (8 epilogue warps) otherwise.
+// tf32 tensor-core implementation of the row-parallel GEMM contract (gemm_args.h) for sm_90a (H100).
+// Persistent, warp-specialised: each CTA loops over 64-row output tiles through a ring of shared-memory stages.  The accumulator of a
+// tile lives in the registers of one consumer warpgroup (wgmma, M = 64, N = 16 per instruction, K = 8).  Two shapes: 2 CTAs / SM for
+// N <= 64 without a prologue, 1 CTA / SM otherwise.
 //
 //   warps 0-3  A producers, three modes:
-//              * TMA (cfg.tma = 1): dense row-major A, one thread issues cp.async.bulk.tensor.2d boxes of 128 rows x 32 floats that
+//              * TMA (cfg.tma = 1): dense row-major A, one thread issues cp.async.bulk.tensor.2d boxes of 64 rows x 32 floats that
 //                land directly in the K-major SWIZZLE_128B layout; rows past M are zero-filled by the unit.
-//              * TMA patches (cfg.tma = 2, template PATCH): same-size convolutions; a tile is a 16 x 8 (h x w) patch of one image and
+//              * TMA patches (cfg.tma = 2, template PATCH): same-size convolutions; a tile is an 8 x 8 (h x w) patch of one image and
 //                a chunk is one (tap, 32 channels) box of a 4-D (C, W, H, B) tensor map with the tap's (dy, dx) added to the
 //                coordinates -- padding is the unit's out-of-bounds zero fill.
-//                With TMA every stage of the ring is in flight; LDGSTS producers saturate near 16 GB/s per SM.
 //              * cp.async (LDGSTS 16 B, zero fill) for strided / transposed convolutions, and LDG -> registers -> transform ->
 //                st.shared for operands with a prologue (BatchNorm+Swish / Swish+dropout / dropout / LayerNorm / InstanceNorm+PReLU).
-//   warp 4     TMEM allocation (2 x N columns); one lane issues tcgen05.mma (kind::tf32, M = 128, N = 16..256, K = 8) and
-//              tcgen05.commit (A-stage release, accumulator ready).
-//   warp 5     weight tiles by cp.async.bulk (UBLKCP) of pre-tiled, pre-swizzled (N x 128 B) blocks: all K chunks once per CTA when
-//              the whole weight fits in shared memory ("resident", every conformer GEMM), else per K chunk through the stage ring
-//              ("streamed", the dilated dense convolutions).
-//   warps 6+   epilogue (compile-time kind): two tcgen05.ld 32x32b.x16 in flight -> per-warp shared-memory staging -> coalesced
-//              float4 rows: bias, dropout, residual, activation gradients, Swish dual output -> global; auxiliary operands are
-//              prefetched one to two 8-row batches ahead; then the accumulator buffer is released.
+//              Thread 0 also issues the weight tiles: cp.async.bulk of pre-tiled, pre-swizzled (N x 128 B) blocks, all K chunks once per
+//              CTA when the whole weight fits in shared memory ("resident", every conformer GEMM), else per K chunk through the stage
+//              ring ("streamed", the dilated dense convolutions).
+//   warps 4-7  consumer warpgroup: wgmma over every K chunk of the tile (stage released when its MMAs have retired), then the epilogue
+//              (compile-time kind): accumulator fragments -> per-warp shared-memory staging -> coalesced float4 rows: bias, dropout,
+//              residual, activation gradients, Swish dual output -> global.
 //
 // The weight operand is re-tiled once per call by pack_b_kernel into the scratch the caller passes (any source layout:
 // Linear (N,K), Conv2d (N,C,kh,kw), and the transposed forms used for data gradients).
@@ -35,16 +32,16 @@ namespace {
 using namespace cmgan_gemm;
 using namespace cmgan_tc;
 
-constexpr int BM = 128;              // rows per tile = UMMA M
+constexpr int BM = 64;               // rows per tile = wgmma M
 constexpr int KC = 32;               // floats per K chunk = one 128-byte swizzle row
-constexpr int A_STAGE_BYTES = BM * KC * 4;   // 16 KB
+constexpr int A_STAGE_BYTES = BM * KC * 4;   // 8 KB
 constexpr int NPROD = 128;           // producer threads (warps 0-3)
-constexpr int NTHREADS4 = 320, NTHREADS8 = 448;     // 4 or 8 epilogue warps
+constexpr int NTHREADS = 256;        // producer warpgroup, consumer warpgroup (two warpgroups: up to 255 registers per thread)
 constexpr int SLAB = 64;             // epilogue column slab
 constexpr int STG_LD = SLAB + 4;     // staging row stride (floats): conflict-free 128-bit accesses
-constexpr int STG_BYTES4 = 4 * 32 * STG_LD * 4;     // 34816: per-warp staging of 32 rows x (64 + 4) floats
-constexpr int STG_BYTES8 = 8 * 32 * STG_LD * 4;
+constexpr int STG_BYTES = 4 * 16 * STG_LD * 4;      // 17408: per-warp staging of 16 rows x (64 + 4) floats
 constexpr int SMEM_LIMIT = 227 * 1024;
+constexpr int SMEM_LIMIT2 = 112 * 1024;             // per CTA when two share an SM
 constexpr int RESIDENT_MAX = 96 * 1024;
 
 // ---- weight re-tiling ------------------------------------------------------------------------------
@@ -78,14 +75,15 @@ __global__ void pack_all_kernel(const CmganPackDesc* __restrict__ descs) {
     }
 }
 
-// tma: 0 = cp.async / register producers, 1 = dense 2-D tensor map, 2 = same-size convolution: tiles are 16 x 8 (h x w) patches of one image
-// (pw = 8 positions along w, ph = 16 lines), fetched through a 4-D tensor map with the tap offset added to the coordinates
-struct TcCfg { int BN, stages, tmem_cols, resident, ntiles, tma, nfx, nty, W, H; };
-constexpr int PW = 8, PH = 16;
+// tma: 0 = cp.async / register producers, 1 = dense 2-D tensor map, 2 = same-size convolution: tiles are 8 x 8 (h x w) patches of one image
+// (pw = 8 positions along w, ph = 8 lines), fetched through a 4-D tensor map with the tap offset added to the coordinates
+struct TcCfg { int BN, stages, resident, ntiles, tma, nfx, nty, W, H; };
+constexpr int PW = 8, PH = 8;
 
-template <bool ASYNC_A, bool EPI8, int EPI, bool PATCH>
-__global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI8) ? 2 : 1) gemm_rows_tc_kernel(const __grid_constant__ CmganGemmArgs g, const float* __restrict__ Bp,
-                                                                    const TcCfg cfg, const __grid_constant__ CUtensorMap tmA) {
+// NBMAX: 16-column blocks the accumulator has room for (4: N <= 64, two CTAs per SM; 16: N <= 256)
+template <bool ASYNC_A, int NBMAX, int EPI, bool PATCH>
+__global__ void __launch_bounds__(NTHREADS, NBMAX == 4 ? 2 : 1) gemm_rows_tc_kernel(const __grid_constant__ CmganGemmArgs g, const float* __restrict__ Bp,
+                                                                                  const TcCfg cfg, const __grid_constant__ CUtensorMap tmA) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;        // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -97,43 +95,45 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
     const uint32_t sB = sA + stages * A_STAGE_BYTES;
     const uint32_t b_region = (uint32_t)(cfg.resident ? nchunks : stages) * b_tile_bytes;
     const uint32_t sStg = sB + b_region;
-    const uint32_t bars = sStg + (EPI8 ? STG_BYTES8 : STG_BYTES4);
+    const uint32_t bars = sStg + STG_BYTES;
     auto full_bar = [&](int s) { return bars + 8u * s; };
     auto empty_bar = [&](int s) { return bars + 8u * (stages + s); };
-    const uint32_t tfull_bar = bars + 8u * (2 * stages);          // [2]
-    const uint32_t tempty_bar = tfull_bar + 16u;                  // [2]
-    const uint32_t bready_bar = tempty_bar + 16u;
-    const uint32_t tmem_ptr_addr = bready_bar + 8u;
+    const uint32_t bready_bar = bars + 8u * (2 * stages);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ntiles = cfg.ntiles;
     const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
     if (tid == 0) {
-        for (int s = 0; s < stages; ++s) { mbar_init(full_bar(s), (cfg.tma ? 1 : NPROD) + (cfg.resident ? 0 : 1)); mbar_init(empty_bar(s), 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar + 8u * b, 1); mbar_init(tempty_bar + 8u * b, EPI8 ? 8 : 4); }
+        for (int s = 0; s < stages; ++s) { mbar_init(full_bar(s), cfg.tma ? 1 : NPROD + (cfg.resident ? 0 : 1)); mbar_init(empty_bar(s), 4); }
         mbar_init(bready_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 4) tmem_alloc(tmem_ptr_addr, (uint32_t)cfg.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_addr));
-    const uint32_t acc_stride = (uint32_t)(cfg.tmem_cols / 2);
 
     if (warp < 4) {
         // ================================ A producers ================================
         const int c = tid & 7;            // 16-byte chunk within the 128-byte row
-        const int rr = tid >> 3;          // rows rr, rr+16, ..., rr+112
-        uint32_t dst_off[8];
+        const int rr = tid >> 3;          // rows rr, rr+16, rr+32, rr+48
+        uint32_t dst_off[4];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) { const int r = rr + 16 * i; dst_off[i] = r * 128 + ((c ^ (r & 7)) << 4); }
+        for (int i = 0; i < 4; ++i) { const int r = rr + 16 * i; dst_off[i] = r * 128 + ((c ^ (r & 7)) << 4); }
         const long total = (long)my_tiles * nchunks;
+        // weight tiles by cp.async.bulk of pre-tiled, pre-swizzled (N x 128 B) blocks, issued by thread 0: all K chunks once when they
+        // fit ("resident"), else one per stage next to the A chunk ("streamed"; B_STAGE is a no-op when resident)
+        if (tid == 0 && cfg.resident) {
+            mbar_arrive_expect_tx(bready_bar, (uint32_t)(nchunks * b_tile_bytes));
+            for (int ch = 0; ch < nchunks; ++ch)
+                bulk_g2s(sB + ch * b_tile_bytes, Bp + (long)ch * BN * KC, (uint32_t)b_tile_bytes, bready_bar);
+        }
+#define B_STAGE(q, s)                                                                                                    \
+        if (tid == 0 && !cfg.resident) {                                                                                 \
+            if (!cfg.tma) mbar_arrive_expect_tx(full_bar(s), (uint32_t)b_tile_bytes);                                    \
+            bulk_g2s(sB + (s) * b_tile_bytes, Bp + (long)((q) % nchunks) * BN * KC, (uint32_t)b_tile_bytes, full_bar(s)); \
+        }
 
         if (ASYNC_A && cfg.tma) {
-            // dense row-major A (no gather): one thread drives TMA, a 128-row x 32-float box per K chunk written straight into the
+            // dense row-major A (no gather): one thread drives TMA, a 64-row x 32-float box per K chunk written straight into the
             // SWIZZLE_128B layout (rows past M are zero-filled by the unit); every stage of the ring can be in flight
             if (tid == 0) {
                 for (long q = 0; q < total; ++q) {
@@ -141,7 +141,8 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                     const int s = (int)(q % stages);
                     const uint32_t par = (uint32_t)((q / stages) & 1);
                     mbar_wait(empty_bar(s), par ^ 1u);
-                    mbar_arrive_expect_tx(full_bar(s), (uint32_t)A_STAGE_BYTES);
+                    mbar_arrive_expect_tx(full_bar(s), (uint32_t)(A_STAGE_BYTES + (cfg.resident ? 0 : b_tile_bytes)));
+                    B_STAGE(q, s)
                     const int tile = blockIdx.x + lt * gridDim.x;
                     if (!PATCH) {
                         tma_load_2d(sA + s * A_STAGE_BYTES, &tmA, ch * KC, tile * BM, full_bar(s));
@@ -155,8 +156,8 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
             __syncwarp();
         } else if (ASYNC_A) {
             const int LAG = stages >= 3 ? 2 : 1;
-            long rowoff[8];
-            RowInfo ri[8];
+            long rowoff[4];
+            RowInfo ri[4];
             int cur_tile = -1, cur_tap = -1;
             for (long q = 0; q < total + LAG; ++q) {
                 if (q < total) {
@@ -168,20 +169,21 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                         cur_tile = lt; cur_tap = -1;
                         const int m0 = (blockIdx.x + lt * gridDim.x) * BM;
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) ri[i] = decode_row(g, m0 + rr + 16 * i);
+                        for (int i = 0; i < 4; ++i) ri[i] = decode_row(g, m0 + rr + 16 * i);
                     }
                     if (tap != cur_tap) {
                         cur_tap = tap;
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) {
+                        for (int i = 0; i < 4; ++i) {
                             long r = in_row_of(g, ri[i], tap);
                             rowoff[i] = r < 0 ? -1 : g.tap_off[tap] + r * g.lda;
                         }
                     }
                     mbar_wait(empty_bar(s), par ^ 1u);
+                    B_STAGE(q, s)
                     const uint32_t sbase = sA + s * A_STAGE_BYTES;
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
+                    for (int i = 0; i < 4; ++i) {
                         const bool ok = rowoff[i] >= 0;
                         cp_async16(sbase + dst_off[i], g.A + (ok ? rowoff[i] + k0 : 0), ok ? 16u : 0u);
                     }
@@ -195,8 +197,8 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                 }
             }
         } else {
-            float mean[8], rstd[8];
-            RowInfo ri[8];
+            float mean[4], rstd[4];
+            RowInfo ri[4];
             int cur_tile = -1;
             for (long q = 0; q < total; ++q) {
                 const int lt = (int)(q / nchunks), ch = (int)(q - (long)lt * nchunks);
@@ -207,7 +209,7 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                     cur_tile = lt;
                     const int m0 = (blockIdx.x + lt * gridDim.x) * BM;
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
+                    for (int i = 0; i < 4; ++i) {
                         ri[i] = decode_row(g, m0 + rr + 16 * i);
                         mean[i] = 0.f; rstd[i] = 1.f;
                         if (g.pro == CMGAN_PRO_LN) {        // ntaps == 1: in_row is constant over the K loop
@@ -218,88 +220,43 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                 }
                 ChunkParams cp;
                 load_chunk_params(g, k0, cp);
-                float4 v[8];
-                long rows[8];
+                float4 v[4];
+                long rows[4];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
+                for (int i = 0; i < 4; ++i) {
                     rows[i] = in_row_of(g, ri[i], tap);
                     v[i] = rows[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(g.A + g.tap_off[tap] + rows[i] * g.lda + k0)) : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
+                for (int i = 0; i < 4; ++i)
                     if (rows[i] >= 0) v[i] = transform4(g, v[i], rows[i], k0, mean[i], rstd[i], cp);
                 mbar_wait(empty_bar(s), par ^ 1u);
+                B_STAGE(q, s)
                 const uint32_t sbase = sA + s * A_STAGE_BYTES;
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
+                for (int i = 0; i < 4; ++i)
                     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + dst_off[i]), "f"(to_tf32(v[i].x)), "f"(to_tf32(v[i].y)),
                                  "f"(to_tf32(v[i].z)), "f"(to_tf32(v[i].w)) : "memory");
                 fence_proxy_async();
                 mbar_arrive(full_bar(s));
             }
         }
-    } else if (warp == 4) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(BM, BN, 0, 0);
-            if (cfg.resident) mbar_wait(bready_bar, 0);
-            long q = 0;
-            for (int lt = 0; lt < my_tiles; ++lt) {
-                const int buf = lt & 1;
-                mbar_wait(tempty_bar + 8u * buf, (uint32_t)(((lt >> 1) & 1) ^ 1));      // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + buf * acc_stride;
-                for (int ch = 0; ch < nchunks; ++ch, ++q) {
-                    const int s = (int)(q % stages);
-                    const uint32_t par = (uint32_t)((q / stages) & 1);
-                    mbar_wait(full_bar(s), par);
-                    tc_fence_after();
-                    const uint64_t adesc = make_desc_sw128(sA + s * A_STAGE_BYTES, 16, 1024);
-                    const uint64_t bdesc = make_desc_sw128(sB + (cfg.resident ? ch : s) * b_tile_bytes, 16, 1024);
-#pragma unroll
-                    for (int k = 0; k < KC / 8; ++k)       // tf32: K = 8 per instruction = 32 bytes along the swizzled row
-                        umma_tf32(tacc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (ch | k) != 0 ? 1u : 0u);
-                    umma_commit(empty_bar(s));             // frees the stage once the MMAs above have read it
-                }
-                umma_commit(tfull_bar + 8u * buf);         // accumulator complete
-            }
-        }
-        __syncwarp();
-    } else if (warp == 5) {
-        // ================================ weight-tile loader (TMA bulk copies) ================================
-        if (lane == 0) {
-            if (cfg.resident) {
-                mbar_arrive_expect_tx(bready_bar, (uint32_t)(nchunks * b_tile_bytes));
-                for (int ch = 0; ch < nchunks; ++ch)
-                    bulk_g2s(sB + ch * b_tile_bytes, Bp + (long)ch * BN * KC, (uint32_t)b_tile_bytes, bready_bar);
-            } else {
-                const long total = (long)my_tiles * nchunks;
-                for (long q = 0; q < total; ++q) {
-                    const int ch = (int)(q % nchunks);
-                    const int s = (int)(q % stages);
-                    const uint32_t par = (uint32_t)((q / stages) & 1);
-                    mbar_wait(empty_bar(s), par ^ 1u);
-                    mbar_arrive_expect_tx(full_bar(s), (uint32_t)b_tile_bytes);
-                    bulk_g2s(sB + s * b_tile_bytes, Bp + (long)ch * BN * KC, (uint32_t)b_tile_bytes, full_bar(s));
-                }
-            }
-        }
-        __syncwarp();
+#undef B_STAGE
     } else {
-        // ================================ epilogue (warps 6-9, or 6-13 with EPI8) ================================
-        // a warp may only touch its TMEM lane quarter (warp % 4); with EPI8 two warps share a quarter and alternate 64-column slabs.
-        // Per slab: 4 x tcgen05.ld in flight -> one wait -> 16 st.shared.v4 (own row) -> the warp re-reads the slab as coalesced
-        // 256-byte row segments (16 lanes x float4, 2 rows per pass), applies the compile-time epilogue and stores.
-        const int q4 = warp & 3;
-        const int ew = warp - 6;
-        const int half = EPI8 ? (ew >> 2) : 0;
-        constexpr int NH = EPI8 ? 2 : 1;
-        constexpr int PD = EPI8 ? 2 : 1;       // auxiliary-operand prefetch distance in batches (register budget: 128 vs 96 per thread)
-        constexpr int RING = EPI8 ? 4 : 2;     // divides the 4 batches of a slab, so slots are compile-time constants
-        float* stg = reinterpret_cast<float*>(base_ptr + (sStg - base)) + ew * 32 * STG_LD;
+        // ================================ consumer warpgroup (warps 4-7): MMAs, then the epilogue ================================
+        // warp cw owns tile rows 16 cw .. 16 cw + 15.  Per 64-column slab: fragments -> st.shared (own rows) -> the warp re-reads the slab
+        // as coalesced 256-byte row segments (16 lanes x float4, 2 rows per pass, 8 passes), applies the compile-time epilogue and stores.
+        const int cw = warp - 4;
+        const int nb = BN / 16;
+        float acc[NBMAX][8];
+#pragma unroll
+        for (int j = 0; j < NBMAX; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) acc[j][i] = 0.f;
+        float* stg = reinterpret_cast<float*>(base_ptr + (sStg - base)) + cw * 16 * STG_LD;
         const int col4 = (lane & 15) * 4;
         const int rsub = lane >> 4;
-        const int nslabs = (BN + SLAB - 1) / SLAB;
+        const int fg = lane >> 2, ft = lane & 3;       // fragment row / column pair
         constexpr bool DROPS = EPI == CMGAN_EPI_DROP_RES || EPI == CMGAN_EPI_DSWISH_DROP || EPI == CMGAN_EPI_SWISH_DUAL;
         const uint32_t seed32 = DROPS ? cmgan_seed32(eff_seed(g)) : 0u;
         const uint32_t thr16 = g.drop_thr >> 16;
@@ -312,66 +269,55 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
         if (EPI == CMGAN_EPI_DROP_RES) { xbase = g.R; ldx = g.ldr; }
         else if (EPI == CMGAN_EPI_DSWISH_DROP || EPI == CMGAN_EPI_DBNSWISH) { xbase = g.aux; ldx = g.ldaux; }
         else if (EPI == CMGAN_EPI_ACC) { xbase = g.C; ldx = g.ldc; }
+        if (cfg.resident) mbar_wait(bready_bar, 0);
+        long q = 0;
         for (int lt = 0; lt < my_tiles; ++lt) {
-            const int buf = lt & 1;
-            // rows of this TMEM lane quarter.  Flat tiles: 32 consecutive rows.  Patch tiles (cfg.tma == 2): 4 image lines x 8 positions.
-            // Pass ps handles quarter rows 2 ps + rsub; its row index is mfirst + (ps >> 2) * hi_rows + 2 * (ps & 3).
+            for (int ch = 0; ch < nchunks; ++ch, ++q) {
+                const int s = (int)(q % stages);
+                const uint32_t par = (uint32_t)((q / stages) & 1);
+                mbar_wait(full_bar(s), par);
+                const uint64_t adesc = gmma_desc_sw128(sA + s * A_STAGE_BYTES);
+                const uint64_t bdesc = gmma_desc_sw128(sB + (cfg.resident ? ch : s) * b_tile_bytes);
+                wgmma_fence();
+                mma_chunk_n<NBMAX>(nb, acc, adesc, bdesc, ch == 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));          // this warp's share of the stage has been read
+            }
+            // rows of this warp.  Flat tiles: 16 consecutive rows.  Patch tiles (cfg.tma == 2): 2 image lines x 8 positions.
+            // Pass ps handles rows 2 ps + rsub; its row index is mfirst + (ps >> 2) * hi_rows + 2 * (ps & 3).
             const int tile = blockIdx.x + lt * gridDim.x;
             long mfirst;
             int hi_rows, vhi, vlo;          // valid: flat: 8 (ps >> 2) + 2 (ps & 3) + rsub < vlo;  patch: (ps >> 2) < vhi && 2 (ps & 3) + rsub < vlo
             if (patch) {
                 const int fx = tile % cfg.nfx, ty = (tile / cfg.nfx) % cfg.nty, bimg = tile / (cfg.nfx * cfg.nty);
-                const int y0 = ty * PH + q4 * 4, x0 = fx * PW;
+                const int y0 = ty * PH + cw * 2, x0 = fx * PW;
                 mfirst = ((long)bimg * cfg.H + y0) * cfg.W + x0 + rsub;
                 hi_rows = cfg.W; vhi = cfg.H - y0; vlo = cfg.W - x0;
             } else {
-                const int mrow0 = tile * BM + q4 * 32;
+                const int mrow0 = tile * BM + cw * 16;
                 mfirst = (long)mrow0 + rsub;
-                hi_rows = 8; vhi = 4; vlo = g.M - mrow0;
+                hi_rows = 8; vhi = 2; vlo = g.M - mrow0;
             }
             auto row_ok = [&](int ps) { return patch ? ((ps >> 2) < vhi && 2 * (ps & 3) + rsub < vlo) : (2 * ps + rsub < vlo); };
             auto row_delta = [&](int ps) { return (long)(ps >> 2) * hi_rows + 2 * (ps & 3); };
             const bool any_row = row_ok(0);
-            // the auxiliary operand does not depend on the accumulator: its first loads are issued before waiting for the MMAs,
-            // later batches (4 passes = 8 rows each) one batch ahead of their use
-            float4 ex[RING][4];                                 // slot = batch index % RING; PD batches of loads in flight
-            auto prefetch = [&](int sl, int b4, float4* dst) {
-                const int n = sl * SLAB + col4;
-                if (xbase == nullptr || n >= BN) return;
-                const float* xp = xbase + mfirst * ldx + n;
 #pragma unroll
-                for (int u = 0; u < 4; ++u)
-                    if (row_ok(b4 * 4 + u)) dst[u] = __ldg(reinterpret_cast<const float4*>(xp + row_delta(b4 * 4 + u) * ldx));
-            };
-            if (half < nslabs) { prefetch(half, 0, ex[0]); if (PD == 2) prefetch(half, 1, ex[1]); }
-            mbar_wait(tfull_bar + 8u * buf, (uint32_t)((lt >> 1) & 1));
-            tc_fence_after();
-            const uint32_t trow = tmem_base + buf * acc_stride + ((uint32_t)(q4 * 32) << 16);
-            bool released = false;
-            for (int sl = half; sl < nslabs; sl += NH) {
+            for (int sl = 0; sl < NBMAX / 4; ++sl) {
                 const int n0 = sl * SLAB;
+                if (n0 >= BN) break;
                 const int ncols = min(SLAB, BN - n0);
 #pragma unroll
-                for (int hq = 0; hq < 2; ++hq) {              // 32 columns at a time: two tcgen05.ld in flight per wait
-                    if (hq * 32 >= ncols) break;
-                    uint32_t r[32];
-                    tmem_ld16_nowait(trow + (uint32_t)(n0 + hq * 32), r);
-                    if (hq * 32 + 16 < ncols) tmem_ld16_nowait(trow + (uint32_t)(n0 + hq * 32 + 16), r + 16);
-                    tmem_wait_ld();
+                for (int jj = 0; jj < 4; ++jj) {
+                    if (16 * jj >= ncols) break;
+                    const float* d = acc[4 * sl + jj];
 #pragma unroll
-                    for (int q = 0; q < 2; ++q)
-                        if (hq * 32 + q * 16 < ncols) {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                *reinterpret_cast<uint4*>(stg + lane * STG_LD + hq * 32 + q * 16 + 4 * j) =
-                                    make_uint4(r[16 * q + 4 * j], r[16 * q + 4 * j + 1], r[16 * q + 4 * j + 2], r[16 * q + 4 * j + 3]);
-                        }
-                }
-                if (sl + NH >= nslabs) {                      // this warp's last slab is out of TMEM: the accumulator buffer may be overwritten
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tempty_bar + 8u * buf);
-                    released = true;
+                    for (int i = 0; i < 2; ++i) {
+                        const int col = 16 * jj + 8 * i + 2 * ft;
+                        *reinterpret_cast<float2*>(stg + fg * STG_LD + col) = make_float2(d[4 * i], d[4 * i + 1]);
+                        *reinterpret_cast<float2*>(stg + (fg + 8) * STG_LD + col) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+                    }
                 }
                 __syncwarp();
                 if (col4 < ncols && any_row) {
@@ -381,14 +327,18 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                     if (EPI == CMGAN_EPI_DBNSWISH) { e0v = __ldg(reinterpret_cast<const float4*>(g.e0 + n)); e1v = __ldg(reinterpret_cast<const float4*>(g.e1 + n)); }
                     float* cptr = g.C ? g.C + mfirst * g.ldc + n : nullptr;
                     float* c2ptr = EPI == CMGAN_EPI_SWISH_DUAL ? g.C2 + mfirst * g.ldc2 + n : nullptr;
+                    const float* xp = xbase ? xbase + mfirst * ldx + n : nullptr;
                     const float* sptr = stg + rsub * STG_LD + col4;
                     const long ldc = g.ldc, ldc2 = g.ldc2;
                     const uint32_t pair = (uint32_t)(((unsigned long long)mfirst * (unsigned long long)g.N + (unsigned long long)n) >> 1);
                     const uint32_t phalf = (uint32_t)g.N >> 1;       // one row further = N / 2 pairs further
 #pragma unroll
-                    for (int b4 = 0; b4 < 4; ++b4) {
-                        if (b4 + PD < 4) prefetch(sl, b4 + PD, ex[(b4 + PD) % RING]);
-                        else if (sl + NH < nslabs) prefetch(sl + NH, b4 + PD - 4, ex[(b4 + PD) % RING]);
+                    for (int b4 = 0; b4 < 2; ++b4) {
+                        float4 ex[4];          // auxiliary operand of the 4 rows of this batch: all loads in flight before the first use
+#pragma unroll
+                        for (int u = 0; u < 4; ++u)
+                            ex[u] = (xp && row_ok(b4 * 4 + u)) ? __ldg(reinterpret_cast<const float4*>(xp + row_delta(b4 * 4 + u) * ldx))
+                                                                : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                         for (int u = 0; u < 4; ++u) {
                             const int ps = b4 * 4 + u;
@@ -403,8 +353,7 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                                 ds[0] = (h0 & 0xFFFFu) >= thr16 ? inv_keep : 0.f; ds[1] = (h0 >> 16) >= thr16 ? inv_keep : 0.f;
                                 ds[2] = (h1 & 0xFFFFu) >= thr16 ? inv_keep : 0.f; ds[3] = (h1 >> 16) >= thr16 ? inv_keep : 0.f;
                             }
-                            const float4 xe = ex[b4 % RING][u];
-                            const float x[4] = {xe.x, xe.y, xe.z, xe.w};
+                            const float x[4] = {ex[u].x, ex[u].y, ex[u].z, ex[u].w};
                             if (EPI == CMGAN_EPI_SWISH_DUAL) {
                                 if (cptr) *reinterpret_cast<float4*>(cptr + rd * ldc) = make_float4(v[0], v[1], v[2], v[3]);
 #pragma unroll
@@ -429,23 +378,10 @@ __global__ void __launch_bounds__(EPI8 ? NTHREADS8 : NTHREADS4, (ASYNC_A && !EPI
                             *reinterpret_cast<float4*>(cptr + rd * ldc) = make_float4(v[0], v[1], v[2], v[3]);
                         }
                     }
-                } else if (sl + NH < nslabs) {
-                    prefetch(sl + NH, 0, ex[0]);
-                    if (PD == 2) prefetch(sl + NH, 1, ex[1]);
                 }
                 __syncwarp();
             }
-            if (!released) {          // no slab for this warp (narrow N): still part of the release count
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty_bar + 8u * buf);
-            }
         }
-    }
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)cfg.tmem_cols);
     }
 }
 
@@ -483,15 +419,15 @@ PFN_encodeTiled get_encoder() {
     return encode;
 }
 
-template <bool ASYNC_A, bool EPI8, int EPI, bool PATCH = false>
+template <bool ASYNC_A, int NBMAX, int EPI, bool PATCH = false>
 int launch_variant(const CmganGemmArgs& a, const TcCfg& cfg, int grid, size_t smem, cudaStream_t st, const CUtensorMap& tm) {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_rows_tc_kernel<ASYNC_A, EPI8, EPI, PATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+        cudaError_t e = cudaFuncSetAttribute(gemm_rows_tc_kernel<ASYNC_A, NBMAX, EPI, PATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
         if (e != cudaSuccess) { cmgan_set_error("gemm_rows_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
         attr_set = true;
     }
-    gemm_rows_tc_kernel<ASYNC_A, EPI8, EPI, PATCH><<<grid, EPI8 ? NTHREADS8 : NTHREADS4, smem, st>>>(a, a.ws, cfg, tm);
+    gemm_rows_tc_kernel<ASYNC_A, NBMAX, EPI, PATCH><<<grid, NTHREADS, smem, st>>>(a, a.ws, cfg, tm);
     return 0;
 }
 
@@ -505,18 +441,15 @@ int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
     const int b_tile = cfg.BN * KC * 4;
     const int nchunks = (a->Cin / KC) * a->ntaps;
     cfg.resident = (long)nchunks * b_tile <= RESIDENT_MAX ? 1 : 0;
-    cfg.tmem_cols = 64;
-    while (cfg.tmem_cols < 2 * cfg.BN) cfg.tmem_cols <<= 1;
-    // configuration A: two co-resident CTAs per SM with 4 epilogue warps each (twice the loads in flight);
-    // configuration B: one CTA per SM with 8 epilogue warps (wide N: TMEM / shared memory allow only one CTA)
+    // two co-resident CTAs per SM when the accumulator is narrow (N <= 64: 32 registers per thread) and no prologue runs in the producers;
+    // otherwise one CTA per SM with the whole shared memory for the ring
     const int resident_bytes = cfg.resident ? nchunks * b_tile : 0;
     const int per_stage = A_STAGE_BYTES + (cfg.resident ? 0 : b_tile);
-    int fixed = 1024 /*alignment*/ + STG_BYTES4 + 256 /*barriers*/ + resident_bytes;
-    int ctas = (a->pro == CMGAN_PRO_NONE && cfg.tmem_cols <= 256 && fixed + 3 * per_stage <= SMEM_LIMIT / 2) ? 2 : 1;
-    const bool epi8 = ctas == 1;
-    if (epi8) fixed += STG_BYTES8 - STG_BYTES4;
-    cfg.stages = (SMEM_LIMIT / ctas - fixed) / per_stage;
-    if (cfg.stages > 6) cfg.stages = 6;
+    const int fixed = 1024 /*alignment*/ + STG_BYTES + 256 /*barriers*/ + resident_bytes;
+    const int ctas = (a->pro == CMGAN_PRO_NONE && cfg.BN <= 64 && fixed + 3 * per_stage <= SMEM_LIMIT2) ? 2 : 1;
+    const bool narrow = ctas == 2;
+    cfg.stages = ((ctas == 2 ? SMEM_LIMIT2 : SMEM_LIMIT) - fixed) / per_stage;
+    if (cfg.stages > 8) cfg.stages = 8;
     if (cfg.stages < 2) return 1;
     cfg.ntiles = cdiv(a->M, BM);
     const size_t smem = (size_t)fixed + (size_t)cfg.stages * per_stage;
@@ -525,7 +458,7 @@ int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
     }
-    // dense row-major A without prologue: describe it to TMA (box = 32 floats x 128 rows, SWIZZLE_128B, zero fill out of bounds)
+    // dense row-major A without prologue: describe it to TMA (box = 32 floats x 64 rows, SWIZZLE_128B, zero fill out of bounds)
     alignas(64) CUtensorMap tm;
     memset(&tm, 0, sizeof(tm));
     cfg.tma = 0;
@@ -543,7 +476,7 @@ int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
             if (r == CUDA_SUCCESS) cfg.tma = 1;
         }
     }
-    // same-size convolution (taps = coordinate offsets of a (C, W, H, B) tensor, padding = out-of-bounds zero fill): 16 x 8 patch tiles
+    // same-size convolution (taps = coordinate offsets of a (C, W, H, B) tensor, padding = out-of-bounds zero fill): 8 x 8 patch tiles
     bool same_off = true;
     for (int t = 1; t < a->ntaps; ++t) same_off = same_off && a->tap_off[t] == a->tap_off[0];
     if (a->pro == CMGAN_PRO_NONE && (a->epi == CMGAN_EPI_NONE || a->epi == CMGAN_EPI_ACC) && a->conv && a->mul_y == 1 && a->mul_x == 1 && a->div_y == 1 && a->div_x == 1 && a->OH == a->IH &&
@@ -572,21 +505,21 @@ int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
         if (cmgan_check_launch("pack_b_kernel")) return -1;
     }
     const int grid = cfg.ntiles < ctas * g_num_sms ? cfg.ntiles : ctas * g_num_sms;
-    const int variant = a->pro != CMGAN_PRO_NONE ? 0 : (epi8 ? 1 : 2);
+    const int variant = a->pro != CMGAN_PRO_NONE ? 0 : (narrow ? 1 : 2);
     int rc = -2;
 #define CMGAN_TC_LAUNCH(E)                                                                                            \
     case E:                                                                                                           \
-        rc = variant == 0   ? launch_variant<false, true, E>(*a, cfg, grid, smem, st, tm)                             \
-             : variant == 1 ? launch_variant<true, true, E>(*a, cfg, grid, smem, st, tm)                              \
-                            : launch_variant<true, false, E>(*a, cfg, grid, smem, st, tm);                            \
+        rc = variant == 0   ? launch_variant<false, 16, E>(*a, cfg, grid, smem, st, tm)                               \
+             : variant == 1 ? launch_variant<true, 4, E>(*a, cfg, grid, smem, st, tm)                                 \
+                            : launch_variant<true, 16, E>(*a, cfg, grid, smem, st, tm);                               \
         break;
     if (cfg.tma == 2) {      // patch tiles (same-size convolutions): forward (plain) and data-gradient (accumulating) epilogues
         if (a->epi == CMGAN_EPI_NONE)
-            rc = epi8 ? launch_variant<true, true, CMGAN_EPI_NONE, true>(*a, cfg, grid, smem, st, tm)
-                      : launch_variant<true, false, CMGAN_EPI_NONE, true>(*a, cfg, grid, smem, st, tm);
+            rc = narrow ? launch_variant<true, 4, CMGAN_EPI_NONE, true>(*a, cfg, grid, smem, st, tm)
+                        : launch_variant<true, 16, CMGAN_EPI_NONE, true>(*a, cfg, grid, smem, st, tm);
         else
-            rc = epi8 ? launch_variant<true, true, CMGAN_EPI_ACC, true>(*a, cfg, grid, smem, st, tm)
-                      : launch_variant<true, false, CMGAN_EPI_ACC, true>(*a, cfg, grid, smem, st, tm);
+            rc = narrow ? launch_variant<true, 4, CMGAN_EPI_ACC, true>(*a, cfg, grid, smem, st, tm)
+                        : launch_variant<true, 16, CMGAN_EPI_ACC, true>(*a, cfg, grid, smem, st, tm);
     } else
     switch (a->epi) {
         CMGAN_TC_LAUNCH(CMGAN_EPI_NONE)

@@ -1,19 +1,11 @@
-// tf32 tensor-core weight gradient:  dW(tap, k, n) += sum_m pro(A[in_row(m, tap), k]) * prod(D[m, n])   (gemm_args.h, wgrad form)
+// tf32 tensor-core weight gradient for sm_90a:  dW(tap, k, n) += sum_m pro(A[in_row(m, tap), k]) * prod(D[m, n])   (gemm_args.h, wgrad form)
 //
-// The reduction runs over the rows m, so both MMA operands are "MN-major": a stage holds 32 rows of A (32 x 128 k) and of D
-// (32 x N) exactly as they lie in memory (rows of 128 B pieces), in the MN-major SWIZZLE_128B_BASE32B layout tf32 requires
-// (descriptor layout type 1): 32-wide M/N blocks 4096 B apart (LBO), 8-row K groups 1024 B apart, 4-row sub-groups 512 B apart
-// (SBO), a row = 128 B whose 32-byte granule q is stored at granule q ^ (row & 3);
-// tcgen05.mma (kind::tf32, M = 128 = k tile, N, K = 8 rows) accumulates the (128 x N) tile of dW in TMEM over a chunk of
-// rows; the epilogue adds the tile into dW with red.global (the parameter-gradient buffer is zeroed once per step).
-// Grid: (row chunks) x (taps * k tiles).  Warps 0-3 load (cp.async when the operand needs no transform, else registers with the
-// same prologues as the forward GEMM / the dropout scale on D) and later run the epilogue; warp 8 issues the MMAs.
-// Bias gradient for free: when Cin is not a multiple of 128 the k tile has spare (zero) rows; the row k = Cin is filled with ones
-// instead, so that accumulator row holds sum_m D[m, n] = dbias.  Otherwise (Cin % 128 == 0, N <= 128) the CTAs of the first k tile issue
-// a second MMA per row group against a constant all-ones A operand into N extra TMEM columns (every row = dbias).  Only N = 256
-// with Cin % 128 == 0 (not on the hot path) still takes the separate colsum_kernel pass.
-#include <cuda.h>      // CUtensorMap (types only; the encoder is fetched from the driver at run time)
-
+// The reduction runs over the rows m, while wgmma reads tf32 operands from shared memory only K-major, so both operands are transposed on
+// their way into shared memory: a stage holds 32 rows as A^T (64 k x 32 m) and D^T (N x 32 m), every line of 32 m-values one 128-byte
+// SWIZZLE_128B row.  One warpgroup per CTA: it stores the next stage (LDG, prologue / dropout scale applied, rounded to tf32) while the MMAs
+// of the current one run (wgmma m64n16k8, 4 K-steps per stage, N / 16 instructions per step), then adds its 64 x N tile into dW with
+// atomics (the parameter-gradient buffer is zeroed once per step).  Grid: (taps x k tiles, row chunks).  The bias gradient is a
+// separate column-sum pass.
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
 #include "gemm_device.cuh"
@@ -23,410 +15,92 @@ namespace {
 using namespace cmgan_gemm;
 using namespace cmgan_tc;
 
-constexpr int RS = 32;               // rows per stage (= 4 MMAs of K = 8)
-constexpr int MO = 128;              // k values per tile = UMMA M
-constexpr int A_STAGE = RS * MO * 4; // 16 KB
-constexpr int NPROD = 256;            // 8 loader warps (warps 0-3 also run the epilogue)
-constexpr int NTHREADS = 288;
-constexpr uint32_t BLK = 4096;       // bytes between 32-wide M/N blocks (4 row groups x 1024)
-__device__ float4 g_ones4 = {1.f, 1.f, 1.f, 1.f};
+constexpr int WT = 128;              // one warpgroup
+constexpr int RS = 32;               // rows per stage = one 128-byte line of m-values
+constexpr int KT = 64;               // k values per tile = wgmma M
+constexpr int A_BYTES = KT * 128;    // 8 KB
 
-__device__ __forceinline__ void advance_row(const CmganGemmArgs& g, RowInfo& r, int by) {
-    r.x += by;
-    if (g.conv) {
-        while (r.x >= g.OW) { r.x -= g.OW; if (++r.y == g.OH) { r.y = 0; ++r.b; } }
-    }
-}
+// byte offset of (line, m) in a K-major SWIZZLE_128B tile of 32-float lines
+__device__ __forceinline__ uint32_t swz(int line, int m) { return (uint32_t)(line * 128 + ((((m >> 2) ^ line) & 7) << 4) + (m & 3) * 4); }
 
-template <bool A_ASYNC, bool D_ASYNC>
-__global__ void __launch_bounds__(NTHREADS, 2) gemm_wgrad_tc_kernel(const __grid_constant__ CmganGemmArgs g, int NB, int mch, int stages,
-                                                                     int tmem_cols) {
+template <int NBMAX>
+__global__ void __launch_bounds__(WT) gemm_wgrad_tc_kernel(const __grid_constant__ CmganGemmArgs g, int mch) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const int d_stage = RS * NB * 4;
-    const uint32_t sA = base;
-    const uint32_t sD = base + stages * A_STAGE;
-    const uint32_t sOnes = sD + stages * d_stage;           // 4 KB of 1.0f (only read when ones_mma), keeps `bars` 8-byte aligned
-    const uint32_t bars = sOnes + 4096;
-    auto full_bar = [&](int s) { return bars + 8u * s; };
-    auto empty_bar = [&](int s) { return bars + 8u * (stages + s); };
-    const uint32_t tmem_full_bar = bars + 8u * (2 * stages);
-    const uint32_t tmem_ptr_addr = tmem_full_bar + 8u;
-
+    uint8_t* const bptr = smem_raw + (base - smem_u32(smem_raw));
+    const int N = g.N, nb = N / 16;
+    const uint32_t stage_bytes = (uint32_t)(A_BYTES + N * 128);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ktiles = (g.Cin + MO - 1) / MO;
-    const int tap = blockIdx.y / ktiles, k0 = (blockIdx.y % ktiles) * MO;
-    const long mbeg = (long)blockIdx.x * mch;
+    const int ktiles = (g.Cin + KT - 1) / KT;
+    const int tap = blockIdx.x / ktiles, k0 = (blockIdx.x % ktiles) * KT;
+    const long mbeg = (long)blockIdx.y * mch;
     const long mend = mbeg + mch < g.M ? mbeg + mch : g.M;
+    const unsigned long long seed = eff_seed(g);
+    // loader lanes: row m = (tid & 7) + 8 i, 4 consecutive columns (k or n) at 4 (tid >> 3) + 64 j -- 2-way bank conflicts on the transposed stores
+    const int lm = tid & 7, lq = (tid >> 3) * 4;
+
+    auto load_stage = [&](long mb, int buf) {
+        uint8_t* sa = bptr + buf * stage_bytes;
+        uint8_t* sd = sa + A_BYTES;
+#pragma unroll
+        for (int i = 0; i < RS / 8; ++i) {
+            const int ml = lm + 8 * i;
+            const long m = mb + ml;
+            RowInfo ri = decode_row(g, (int)(m < mend ? m : g.M));
+            if (m >= mend) ri.ok = false;
+            float a[4];
+            load_a4<4>(g, in_row_of(g, ri, tap), tap, k0 + lq, a);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) *reinterpret_cast<float*>(sa + swz(lq + j, ml)) = to_tf32(a[j]);
+            for (int n = lq; n < N; n += 64) {
+                float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (m < mend) d = __ldg(reinterpret_cast<const float4*>(g.D + m * g.ldd + n));
+                float dv[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    if (g.prod == 1 && m < mend) dv[j] *= g.alpha * cmgan_drop_scale(seed, (uint64_t)m * N + n + j, g.drop_thr, g.inv_keep);
+                    *reinterpret_cast<float*>(sd + swz(n + j, ml)) = to_tf32(dv[j]);
+                }
+            }
+        }
+        fence_proxy_async();          // generic-proxy stores -> visible to the tensor core's async proxy
+    };
+
+    float acc[NBMAX][8];
+#pragma unroll
+    for (int j = 0; j < NBMAX; ++j)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[j][i] = 0.f;
     const int nst = (int)((mend - mbeg + RS - 1) / RS);
-    const bool ones_mma = g.dbias != nullptr && g.Cin % MO == 0 && 2 * NB <= tmem_cols && blockIdx.y == 0;
-    if (ones_mma) {
-        for (int i = threadIdx.x; i < 1024; i += NTHREADS) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sOnes + 4u * i), "f"(1.0f) : "memory");
-        fence_proxy_async();
-    }
-
-    if (tid == 0) {
-        for (int s = 0; s < stages; ++s) { mbar_init(full_bar(s), NPROD); mbar_init(empty_bar(s), 1); }
-        mbar_init(tmem_full_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 8) tmem_alloc(tmem_ptr_addr, (uint32_t)tmem_cols);
-    tc_fence_before();
+    if (nst > 0) load_stage(mbeg, 0);
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_addr));
-
-    if (warp < 8) {
-        // ---------------- producers ----------------
-        // A: thread -> 16-byte chunk j of k block mi, rows rg*4 .. rg*4+3 of the stage
-        const int aj = tid & 7, ami = (tid >> 3) & 3, arg = tid >> 5;
-        const int ak = k0 + ami * 32 + aj * 4;
-        const bool ak_ok = ak < g.Cin;
-        const bool ones_col = g.dbias != nullptr && tap == 0 && ak == g.Cin;      // this thread's chunk starts at the spare row k = Cin
-        uint32_t a_off[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) a_off[i] = ami * BLK + (arg * 4 + i) * 128 + ((((aj >> 1) ^ i) << 5) | ((aj & 1) << 4));
-        RowInfo r0 = decode_row(g, (int)(mbeg + arg * 4));
-        ChunkParams cp;
-        cp.a = cp.b = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (!A_ASYNC && ak_ok) load_chunk_params(g, ak, cp);
-        // D: chunks q = tid + 256 u,  u < NB/32
-        const int cpr = NB / 4;
-        const int nd = NB / 32;
-        const int LAG = stages >= 3 ? 2 : 1;
-        constexpr bool ANY_ASYNC = A_ASYNC || D_ASYNC;
-
-        for (int it = 0; it < nst + (ANY_ASYNC ? LAG : 0); ++it) {
-            if (it < nst) {
-                const int s = it % stages;
-                const uint32_t par = (uint32_t)((it / stages) & 1);
-                const long mrow = mbeg + (long)it * RS;
-                // ---- gather the 8 A rows of this thread (registers or addresses)
-                long arow[4];
-                {
-                    RowInfo r = r0;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const long m = mrow + arg * 4 + i;
-                        r.ok = m < mend;
-                        arow[i] = in_row_of(g, r, tap);
-                        advance_row(g, r, 1);
-                    }
-                    advance_row(g, r0, RS);
-                }
-                float4 av[4];
-                if (!A_ASYNC) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        av[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (arow[i] >= 0 && ak_ok) {
-                            av[i] = __ldg(reinterpret_cast<const float4*>(g.A + g.tap_off[tap] + arow[i] * g.lda + ak));
-                            float mean = 0.f, rstd = 1.f;
-                            if (g.pro == CMGAN_PRO_LN) { float2 st = __ldg(reinterpret_cast<const float2*>(g.p0) + arow[i]); mean = st.x; rstd = st.y; }
-                            av[i] = transform4(g, av[i], arow[i], ak, mean, rstd, cp);
-                        }
-                    }
-                }
-                float4 dv[8];
-                if (!D_ASYNC) {
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) {
-                        if (u < nd) {
-                            const int q = tid + 256 * u;
-                            const int row = q / cpr, cc = q % cpr;
-                            const long m = mrow + row;
-                            dv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (m < mend) {
-                                dv[u] = __ldg(reinterpret_cast<const float4*>(g.D + m * g.ldd + cc * 4));
-                                if (g.prod == 1) {
-                                    float ds[4];
-                                    cmgan_drop_scale4(eff_seed(g), (uint64_t)m * g.N + cc * 4, g.drop_thr, g.inv_keep, ds);
-                                    dv[u].x *= g.alpha * ds[0]; dv[u].y *= g.alpha * ds[1]; dv[u].z *= g.alpha * ds[2]; dv[u].w *= g.alpha * ds[3];
-                                }
-                            }
-                        }
-                    }
-                }
-                mbar_wait(empty_bar(s), par ^ 1u);
-                const uint32_t abase = sA + s * A_STAGE, dbase = sD + s * d_stage;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    if (A_ASYNC) {
-                        const bool ok = arow[i] >= 0 && ak_ok;
-                        const float* src = ones_col ? reinterpret_cast<const float*>(&g_ones4) : g.A + (ok ? g.tap_off[tap] + arow[i] * g.lda + ak : 0);
-                        cp_async16(abase + a_off[i], src, (ok || ones_col) ? 16u : 0u);
-                    } else {
-                        if (ones_col) av[i] = make_float4(1.f, 1.f, 1.f, 1.f);
-                        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(abase + a_off[i]), "f"(to_tf32(av[i].x)), "f"(to_tf32(av[i].y)),
-                                     "f"(to_tf32(av[i].z)), "f"(to_tf32(av[i].w)) : "memory");
-                    }
-                }
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    if (u < nd) {
-                        const int q = tid + 256 * u;
-                        const int row = q / cpr, cc = q % cpr;
-                        const uint32_t off = (uint32_t)(cc >> 3) * BLK + row * 128 + (((((cc & 7) >> 1) ^ (row & 3)) << 5) | ((cc & 1) << 4));
-                        if (D_ASYNC) {
-                            const long m = mrow + row;
-                            const bool ok = m < mend;
-                            cp_async16(dbase + off, g.D + (ok ? m * g.ldd + cc * 4 : 0), ok ? 16u : 0u);
-                        } else {
-                            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dbase + off), "f"(to_tf32(dv[u].x)), "f"(to_tf32(dv[u].y)),
-                                         "f"(to_tf32(dv[u].z)), "f"(to_tf32(dv[u].w)) : "memory");
-                        }
-                    }
-                }
-                if (!ANY_ASYNC) { fence_proxy_async(); mbar_arrive(full_bar(s)); }
-            }
-            if (ANY_ASYNC) {
-                cp_async_commit();
-                const int done = it - LAG;
-                if (done >= 0) {
-                    if (LAG == 2) cp_async_wait<2>(); else cp_async_wait<1>();
-                    fence_proxy_async();
-                    mbar_arrive(full_bar(done % stages));
-                }
-            }
-        }
-        // ---------------- epilogue: dW tile += accumulator (warps 0-3: one TMEM lane quarter each) ----------------
-        if (warp < 4) {
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        const int k = k0 + warp * 32 + lane;
-        const bool bias_row = g.dbias != nullptr && tap == 0 && k == g.Cin;
-        const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-        for (int n0 = 0; n0 < NB; n0 += 16) {
-            float acc[16];
-            tmem_ld16(trow + (uint32_t)n0, acc);
-            if (bias_row) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n0 + j < g.N) atomicAdd(g.dbias + n0 + j, acc[j]);
-            }
-            if (k < g.Cin) {
-                float* dst = g.C + (long)tap * g.sb_tap + (long)k * g.sb_k;
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n0 + j < g.N) atomicAdd(dst + (long)(n0 + j) * g.sb_n, acc[j]);
-            }
-        }
-        if (ones_mma && warp == 0) {              // every row of the second accumulator is the column sum of D
-            for (int n0 = 0; n0 < NB; n0 += 16) {
-                float acc[16];
-                tmem_ld16(trow + (uint32_t)(NB + n0), acc);
-                if (lane == 0) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (n0 + j < g.N) atomicAdd(g.dbias + n0 + j, acc[j]);
-                }
-            }
-        }
-        tc_fence_before();
-        }
-    } else {
-        // ---------------- MMA issuer ----------------
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(MO, NB, 1, 1);
-            for (int it = 0; it < nst; ++it) {
-                const int s = it % stages;
-                const uint32_t par = (uint32_t)((it / stages) & 1);
-                mbar_wait(full_bar(s), par);
-                tc_fence_after();
-#pragma unroll
-                for (int kb = 0; kb < RS / 8; ++kb) {
-                    const uint64_t adesc = make_desc_sw128(sA + s * A_STAGE + kb * 1024, BLK, 512, 1);
-                    const uint64_t ddesc = make_desc_sw128(sD + s * d_stage + kb * 1024, BLK, 512, 1);
-                    umma_tf32(tmem_base, adesc, ddesc, idesc, (it | kb) != 0 ? 1u : 0u);
-                    if (ones_mma)       // A = ones (4 blocks of 8 rows x 128 B, 1 KB apart): accumulator rows = column sums of D
-                        umma_tf32(tmem_base + (uint32_t)NB, make_desc_sw128(sOnes, 1024, 512, 1), ddesc, idesc, (it | kb) != 0 ? 1u : 0u);
-                }
-                umma_commit(empty_bar(s));
-            }
-            umma_commit(tmem_full_bar);
-        }
-        __syncwarp();
+    for (int st = 0; st < nst; ++st) {
+        const uint32_t sa = base + (st & 1) * stage_bytes;
+        wgmma_fence();
+        mma_chunk_n<NBMAX>(nb, acc, gmma_desc_sw128(sa), gmma_desc_sw128(sa + A_BYTES), st == 0);
+        wgmma_commit();
+        if (st + 1 < nst) load_stage(mbeg + (long)(st + 1) * RS, (st + 1) & 1);     // the other buffer: its MMAs retired last iteration
+        wgmma_wait<0>();
+        __syncthreads();
     }
-    __syncthreads();
-    if (warp == 8) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)tmem_cols);
-    }
-}
-
-
-// ---- plain operands (no prologue, plain D; dense rows or a same-size convolution gather): both operands by TMA.
-// A box = 32 rows x 32 floats lands as one (row, 128 B) block of the MN-major SWIZZLE_128B_BASE32B layout (tensor-map swizzle
-// 128B_ATOM_32B), so a stage is 4 boxes of A (k blocks) + N/32 boxes of D, issued by one thread with the whole ring in flight
-// (cp.async tops out near a third of HBM rate per SM).  The activation is described as a (C, W, H, B) tensor and a stage is 32
-// consecutive positions of one image line: the tap's (dy, dx) is added to the box coordinates and the unit zero-fills whatever
-// falls outside the image (the convolution's padding) or past the line end; a dense matrix is the one-line case (W = M).
-// k blocks past Cin are never loaded: they are initialised once (zeros, or ones in row k = Cin for the bias gradient).
-// Warps 0-3 epilogue, warp 4 TMA producer, warp 5 TMEM allocation + MMA issue.
-constexpr int NT_TMA = 192;
-__global__ void __launch_bounds__(NT_TMA, 2) gemm_wgrad_tma_kernel(const __grid_constant__ CmganGemmArgs g, int NB, int ipc, int stages,
-                                                                   int tmem_cols, int items, int fblocks, int lines_h,
-                                                                   const __grid_constant__ CUtensorMap tmA,
-                                                                   const __grid_constant__ CUtensorMap tmD) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const int d_stage = RS * NB * 4;
-    const uint32_t sA = base;
-    const uint32_t sD = base + stages * A_STAGE;
-    const uint32_t sOnes = sD + stages * d_stage;
-    const uint32_t bars = sOnes + 4096;
-    auto full_bar = [&](int s) { return bars + 8u * s; };
-    auto empty_bar = [&](int s) { return bars + 8u * (stages + s); };
-    const uint32_t tmem_full_bar = bars + 8u * (2 * stages);
-    const uint32_t tmem_ptr_addr = tmem_full_bar + 8u;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ktiles = (g.Cin + MO - 1) / MO;
-    const int tap = blockIdx.y / ktiles, k0 = (blockIdx.y % ktiles) * MO;
-    const int kblk = min(4, (g.Cin - k0) / 32);              // valid 32-wide k blocks of this tile (Cin % 32 == 0)
-    const int ibeg = blockIdx.x * ipc;                       // items = (image line, block of 32 positions)
-    const int nst = min(ipc, items - ibeg);
-    const bool spare_row = g.dbias != nullptr && kblk < 4 && tap == 0;   // accumulator row k = Cin collects sum_m D[m, :]
-    const bool ones_mma = g.dbias != nullptr && g.Cin % MO == 0 && 2 * NB <= tmem_cols && blockIdx.y == 0;
-
-    // k blocks never touched by TMA: zeros, except (bias gradient) 1.0 at k = Cin for every row of the stage
-    for (int i = tid; i < stages * (4 - kblk) * 1024; i += NT_TMA) {
-        const int s = i / ((4 - kblk) * 1024), rem = i % ((4 - kblk) * 1024);
-        const int blk = kblk + rem / 1024, w = rem % 1024;       // w = float index inside the 4 KB block: row = w / 32
-        const int row = w >> 5, pos = w & 31;
-        const float v = (spare_row && blk == kblk && pos == ((row & 3) << 3)) ? 1.0f : 0.0f;     // element k = Cin sits in granule 0 ^ (row & 3)
-        reinterpret_cast<float*>(base_ptr + (sA - base) + (size_t)s * A_STAGE + (size_t)blk * BLK)[w] = v;
-    }
-    if (ones_mma)
-        for (int i = tid; i < 1024; i += NT_TMA) reinterpret_cast<float*>(base_ptr + (sOnes - base))[i] = 1.0f;
-    fence_proxy_async();
-    if (tid == 0) {
-        for (int s = 0; s < stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        mbar_init(tmem_full_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 5) tmem_alloc(tmem_ptr_addr, (uint32_t)tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_addr));
-
-    if (warp == 4) {
-        if (lane == 0) {
-            const uint32_t tx = (uint32_t)(kblk + NB / 32) * BLK;
-            const int dy = g.conv ? g.dy[tap] : 0, dx = g.conv ? g.dx[tap] : 0;
-            for (int it = 0; it < nst; ++it) {
-                const int s = it % stages;
-                const uint32_t par = (uint32_t)((it / stages) & 1);
-                const int item = ibeg + it;
-                const int line = item / fblocks, x0 = (item - line * fblocks) * RS;
-                const int bimg = line / lines_h, y = line - bimg * lines_h;
-                mbar_wait(empty_bar(s), par ^ 1u);
-                mbar_arrive_expect_tx(full_bar(s), tx);
-                for (int b = 0; b < kblk; ++b) tma_load_4d(sA + s * A_STAGE + b * BLK, &tmA, k0 + b * 32, x0 + dx, y + dy, bimg, full_bar(s));
-                for (int b = 0; b < NB / 32; ++b) tma_load_3d(sD + s * d_stage + b * BLK, &tmD, b * 32, x0, line, full_bar(s));
-            }
-        }
-        __syncwarp();
-    } else if (warp == 5) {
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(MO, NB, 1, 1);
-            for (int it = 0; it < nst; ++it) {
-                const int s = it % stages;
-                const uint32_t par = (uint32_t)((it / stages) & 1);
-                mbar_wait(full_bar(s), par);
-                tc_fence_after();
+    if (nst == 0) return;
+    // fragment of warp w: k = k0 + 16 w + lane / 4 (+ 8), n = 16 j + 8 i + 2 (lane % 4) (+ 1)
+    const int kr = k0 + 16 * warp + (lane >> 2), nc = 2 * (lane & 3);
+    float* const dst = g.C + (long)tap * g.sb_tap;
 #pragma unroll
-                for (int kb = 0; kb < RS / 8; ++kb) {
-                    const uint64_t adesc = make_desc_sw128(sA + s * A_STAGE + kb * 1024, BLK, 512, 1);
-                    const uint64_t ddesc = make_desc_sw128(sD + s * d_stage + kb * 1024, BLK, 512, 1);
-                    umma_tf32(tmem_base, adesc, ddesc, idesc, (it | kb) != 0 ? 1u : 0u);
-                    if (ones_mma)
-                        umma_tf32(tmem_base + (uint32_t)NB, make_desc_sw128(sOnes, 1024, 512, 1), ddesc, idesc, (it | kb) != 0 ? 1u : 0u);
-                }
-                umma_commit(empty_bar(s));
-            }
-            umma_commit(tmem_full_bar);
-        }
-        __syncwarp();
-    } else {
-        // ---------------- epilogue: dW tile += accumulator (one TMEM lane quarter per warp) ----------------
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        const int k = k0 + warp * 32 + lane;
-        const bool bias_row = spare_row && k == g.Cin;
-        const bool bias_warp = spare_row && (g.Cin - k0) / 32 == warp;          // the warp whose lane 0 holds accumulator row k = Cin
-        // the bias row is staged in shared memory and added with full-line red.global: single-lane atomics from ~300 CTAs onto the
-        // same 8 cache lines serialise (~20 us); a warp-wide add of 32 consecutive floats is one L2 operation per line
-        float* bscr = reinterpret_cast<float*>(base_ptr + (sOnes - base));      // the ones block is dead once the accumulators are complete
-        const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-        for (int n0 = 0; n0 < NB; n0 += 16) {
-            float acc[16];
-            tmem_ld16(trow + (uint32_t)n0, acc);
-            if (bias_row) {
+    for (int j = 0; j < NBMAX; ++j) {
+        if (j >= nb) break;
 #pragma unroll
-                for (int j = 0; j < 16; ++j) bscr[n0 + j] = acc[j];
-            }
-            if (k < g.Cin) {
-                float* dst = g.C + (long)tap * g.sb_tap + (long)k * g.sb_k;
+        for (int i = 0; i < 2; ++i)
 #pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n0 + j < g.N) atomicAdd(dst + (long)(n0 + j) * g.sb_n, acc[j]);
+            for (int h = 0; h < 2; ++h) {
+                const int k = kr + 8 * h;
+                if (k >= g.Cin) continue;
+                const int n = 16 * j + 8 * i + nc;
+                atomicAdd(dst + (long)k * g.sb_k + (long)n * g.sb_n, acc[j][4 * i + 2 * h]);
+                atomicAdd(dst + (long)k * g.sb_k + (long)(n + 1) * g.sb_n, acc[j][4 * i + 2 * h + 1]);
             }
-        }
-        if (bias_warp) {
-            __syncwarp();
-            for (int n = lane; n < g.N; n += 32) atomicAdd(g.dbias + n, bscr[n]);
-        }
-        if (ones_mma && warp == 0) {
-            for (int n0 = 0; n0 < NB; n0 += 16) {
-                float acc[16];
-                tmem_ld16(trow + (uint32_t)(NB + n0), acc);
-                if (lane == 0) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) bscr[n0 + j] = acc[j];
-                }
-            }
-            __syncwarp();
-            for (int n = lane; n < g.N; n += 32) atomicAdd(g.dbias + n, bscr[n]);
-        }
-        tc_fence_before();
     }
-    __syncthreads();
-    if (warp == 5) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)tmem_cols);
-    }
-}
-
-using PFN_encodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                      const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled get_encoder() {
-    static PFN_encodeTiled encode = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            encode = reinterpret_cast<PFN_encodeTiled>(fn);
-    }
-    return encode;
-}
-// fp32 rows of `cols` floats (leading dimension ld) indexed (x < W, y < H, b < B) [rank 4] or (x < W, line < H) [rank 3]; boxes of
-// 32 floats x 32 positions of one line; MN-major SWIZZLE_128B_BASE32B image in shared memory
-bool make_map32(CUtensorMap* tm, int rank, const float* ptr, long long cols, long long W, long long H, long long B, long long ld) {
-    PFN_encodeTiled enc = get_encoder();
-    if (!enc) return false;
-    const cuuint64_t gdim[4] = {(cuuint64_t)cols, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    const cuuint64_t gstride[3] = {(cuuint64_t)ld * sizeof(float), (cuuint64_t)W * ld * sizeof(float), (cuuint64_t)H * W * ld * sizeof(float)};
-    const cuuint32_t box[4] = {32, 32, 1, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<float*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // dbias[n] += sum_m prod(D[m, n])
@@ -454,89 +128,42 @@ __global__ void colsum_kernel(const float* __restrict__ D, long ldd, long M, int
 }
 
 int wgrad_tc_supported(const CmganGemmArgs* a) {
-    if (a->N % 32 || a->N < 32 || a->N > 256) return 0;
-    if (a->Cin % 4) return 0;
-    if (a->lda % 4 || ((uintptr_t)a->A & 15) || a->ldd % 4 || ((uintptr_t)a->D & 15)) return 0;
+    if (a->N % 16 || a->N < 16 || a->N > 256) return 0;
+    if (a->Cin % 4 || a->lda % 4 || ((uintptr_t)a->A & 15) || a->ldd % 4 || ((uintptr_t)a->D & 15)) return 0;
     for (int t = 0; t < a->ntaps; ++t)
         if (a->tap_off[t] % 4) return 0;
-    if (a->pro == CMGAN_PRO_LN && (((uintptr_t)a->p1 & 15) || ((uintptr_t)a->p2 & 15))) return 0;
-    if (a->pro == CMGAN_PRO_BN_SWISH && (((uintptr_t)a->p0 & 15) || ((uintptr_t)a->p1 & 15))) return 0;
-    if (a->pro == CMGAN_PRO_IN_PRELU) return 0;
     return 1;
 }
 
-template <bool AA, bool DA>
-int launch(const CmganGemmArgs* a, dim3 grid, size_t smem, int NB, int mch, int stages, int tmem_cols, cudaStream_t st) {
+template <int NBMAX>
+int launch(const CmganGemmArgs* a, dim3 grid, size_t smem, int mch, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_tc_kernel<AA, DA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(110 * 1024));
+        cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_tc_kernel<NBMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 1024));
         if (e != cudaSuccess) { cmgan_set_error("gemm_wgrad_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
         attr_set = true;
     }
-    gemm_wgrad_tc_kernel<AA, DA><<<grid, NTHREADS, smem, st>>>(*a, NB, mch, stages, tmem_cols);
+    gemm_wgrad_tc_kernel<NBMAX><<<grid, WT, smem, st>>>(*a, mch);
     return cmgan_check_launch("gemm_wgrad_tc_kernel");
 }
 
 }  // namespace
 
-// tf32 tensor-core path of cmgan_gemm_wgrad (same contract).  Returns 1 if the shape is not covered (caller falls back).
+// tf32 tensor-core path of cmgan_gemm_wgrad (same contract).  Returns 1 if the shape is not covered (caller runs the fp32 kernels).
 int cmgan_gemm_wgrad_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
     if (!wgrad_tc_supported(a)) return 1;
-    const int NB = a->N;
-    const int d_stage = RS * NB * 4;
-    int stages = (100 * 1024 - 2048 - 4096) / (A_STAGE + d_stage);
-    if (stages > 4) stages = 4;
-    if (stages < 2) stages = 2;
-    const bool ones_mma = a->dbias && a->Cin % MO == 0 && NB <= 128;      // 2 N columns, two co-resident CTAs -> N <= 128
-    int tmem_cols = 32;
-    while (tmem_cols < (ones_mma ? 2 * NB : NB)) tmem_cols <<= 1;
-    const int ktiles = (a->Cin + MO - 1) / MO;
-    const int ytiles = ktiles * a->ntaps;
-    // rows per CTA: one full wave of 2 co-resident CTAs per SM (every CTA ends with one red.global pass over its dW tile, so more,
-    // smaller CTAs only add atomics and a ragged second wave), at least 8 stages per CTA
-    int sms = 148;
-    {
-        int dev = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    long want = (2L * sms) / ytiles;
+    const int ytiles = ((a->Cin + KT - 1) / KT) * a->ntaps;
+    // rows per CTA: about four resident CTAs per SM in one wave (every CTA ends with one atomic pass over its dW tile), at least 8 stages
+    long want = (4L * cmgan_num_sms()) / ytiles;
     if (want < 1) want = 1;
     long mch = (a->M + want - 1) / want;
     mch = ((mch + RS - 1) / RS) * RS;
     if (mch < 8 * RS) mch = 8 * RS;
-    dim3 grid((unsigned)((a->M + mch - 1) / mch), (unsigned)ytiles);
-    const size_t smem = (size_t)stages * (A_STAGE + d_stage) + 4096 + 1024 + 8 * (2 * stages + 2) + 16;
-    const bool aa = a->pro == CMGAN_PRO_NONE, da = a->prod == 0;
-    int rc;
-    alignas(64) CUtensorMap tmA, tmD;
-    // TMA path: dense rows, or a convolution whose output grid equals its input grid (taps = coordinate offsets, padding = OOB fill)
-    bool same_off = true;
-    for (int t = 1; t < a->ntaps; ++t) same_off = same_off && a->tap_off[t] == a->tap_off[0];
-    const bool dense = !a->conv && a->ntaps == 1;
-    const bool conv_same = a->conv && a->mul_y == 1 && a->mul_x == 1 && a->div_y == 1 && a->div_x == 1 && a->OH == a->IH && a->OW == a->IW &&
-                           same_off && a->M % ((long long)a->OH * a->OW) == 0;
-    const long long W = dense ? a->M : a->OW, Hh = dense ? 1 : a->OH, Bn = dense ? 1 : a->M / ((long long)a->OH * a->OW);
-    const long long fblocks = (W + RS - 1) / RS, items = Hh * Bn * fblocks;
-    if (aa && da && (dense || conv_same) && a->Cin % 32 == 0 && items < (1ll << 30) &&
-        make_map32(&tmA, 4, a->A + a->tap_off[0], a->Cin, W, Hh, Bn, a->lda) && make_map32(&tmD, 3, a->D, a->N, W, Hh * Bn, 1, a->ldd)) {
-        static bool attr_set = false;
-        if (!attr_set) {
-            cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(110 * 1024));
-            if (e != cudaSuccess) { cmgan_set_error("gemm_wgrad_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
-            attr_set = true;
-        }
-        long long ipc = (items + want - 1) / want;       // items per CTA: one full wave
-        if (ipc < 8) ipc = 8;
-        dim3 grid_t((unsigned)((items + ipc - 1) / ipc), (unsigned)ytiles);
-        gemm_wgrad_tma_kernel<<<grid_t, NT_TMA, smem, st>>>(*a, NB, (int)ipc, stages, tmem_cols, (int)items, (int)fblocks, (int)Hh, tmA, tmD);
-        rc = cmgan_check_launch("gemm_wgrad_tma_kernel");
-    } else
-    if (aa && da) rc = launch<true, true>(a, grid, smem, NB, (int)mch, stages, tmem_cols, st);
-    else if (aa) rc = launch<true, false>(a, grid, smem, NB, (int)mch, stages, tmem_cols, st);
-    else if (da) rc = launch<false, true>(a, grid, smem, NB, (int)mch, stages, tmem_cols, st);
-    else rc = launch<false, false>(a, grid, smem, NB, (int)mch, stages, tmem_cols, st);
+    const dim3 grid((unsigned)ytiles, (unsigned)((a->M + mch - 1) / mch));
+    const size_t smem = 1024 + 2 * (size_t)(A_BYTES + a->N * 128);
+    const int rc = a->N <= 64 ? launch<4>(a, grid, smem, (int)mch, st) : launch<16>(a, grid, smem, (int)mch, st);
     if (rc) return rc;
-    if (a->dbias && a->Cin % MO == 0 && !ones_mma) {       // no spare accumulator row, too wide for the ones MMA
+    if (a->dbias) {
         const int rpb = 64 * (256 / a->N > 0 ? 256 / a->N : 1);     // ~64 rows per thread -> thousands of blocks
         colsum_kernel<<<cdiv(a->M, rpb), 256, 0, st>>>(a->D, a->ldd, a->M, a->N, a->prod, a->alpha, a->seed, a->drop_thr, a->inv_keep, rpb, a->dbias, a->seed_dev);
         return cmgan_check_launch("colsum_kernel");

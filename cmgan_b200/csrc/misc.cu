@@ -26,6 +26,15 @@ int cmgan_check_launch(const char* what) {
     return 0;
 }
 
+int cmgan_num_sms() {
+    static int n = 0;
+    if (n == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    }
+    return n;
+}
+
 CMGAN_API const char* cmgan_last_error(void) { return g_err; }
 CMGAN_API int cmgan_abi_version(void) { return 1; }
 CMGAN_API int cmgan_gemm_args_size(void) { return (int)sizeof(CmganGemmArgs); }

@@ -1,5 +1,5 @@
-// PTX wrappers for the Blackwell (sm_100a) tensor-core kernels: mbarrier, cp.async / cp.async.bulk, tcgen05 (alloc, mma,
-// commit, ld, fences) and the UMMA shared-memory / instruction descriptors (bit layouts follow cute/arch/mma_sm100_desc.hpp).
+// PTX wrappers for the Hopper (sm_90a) tensor-core kernels: mbarrier, cp.async / cp.async.bulk / TMA, wgmma and its shared-memory
+// matrix descriptor (bit layout: PTX ISA, "Matrix Descriptor Format" of the asynchronous warpgroup-level MMA).
 #pragma once
 #include "common.cuh"
 
@@ -33,8 +33,6 @@ __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -60,68 +58,53 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float v[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// issue only (pair with tmem_wait_ld): several loads can be in flight before one wait
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t r[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-}
-// same, straight into float registers (no copy through a second array)
-__device__ __forceinline__ void tmem_ld16f_nowait(uint32_t taddr, float r[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7]), "=f"(r[8]), "=f"(r[9]),
-                   "=f"(r[10]), "=f"(r[11]), "=f"(r[12]), "=f"(r[13]), "=f"(r[14]), "=f"(r[15])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
 }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1), SWIZZLE_128B.
-//   K-major operand  (rows = M/N index, 128 B = 32 tf32 along K): lbo unused (1), sbo = 1024 (next 8-row group)
-//   MN-major operand (rows = K index, 128 B = 32 tf32 along M/N):  lbo = byte distance between 32-wide M/N blocks,
-//                                                                  sbo = byte distance between 8-row K groups
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2) {
+// wgmma (sm_90a warpgroup MMA).  Shared-memory matrix descriptor for a K-major SWIZZLE_128B operand (rows = M/N index, 128 B = 32 tf32
+// along K, 8-row groups 1024 B apart; the tile must start on a 1024-byte boundary): leading byte offset unused (1), stride byte offset 1024.
+// Advancing K by 8 tf32 (one instruction) = +32 bytes = +2 in the address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
     uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);            // start address            bits [0,14)
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // leading byte offset >> 4 bits [16,30)
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;   // stride byte offset >> 4  bits [32,46)
-    d |= (uint64_t)1 << 46;                             // descriptor version (sm_100)
-    d |= (uint64_t)layout_type << 61;                   // 2 = SWIZZLE_128B (16-byte chunks), 1 = SWIZZLE_128B_BASE32B (32-byte chunks)
+    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);            // start address >> 4         bits [0,14)
+    d |= (uint64_t)1 << 16;                             // leading byte offset >> 4   bits [16,30)
+    d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset >> 4    bits [32,46)
+    d |= (uint64_t)1 << 62;                             // layout type 1 = SWIZZLE_128B
     return d;
 }
-// cute::UMMA::InstrDescriptor for kind::tf32 with fp32 accumulation; a_mn / b_mn = 1 for MN-major operands
-__device__ __forceinline__ uint32_t make_idesc_tf32(int M, int N, int a_mn, int b_mn) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 16] (+)= A[64 x 8] B[16 x 8]^T, tf32 operands from shared memory, fp32 accumulators in registers.  Fragment of warp w of the
+// warpgroup, lane l: d[4 i + 0 / 1] = row 16 w + l / 4, columns 8 i + 2 (l % 4) + 0 / 1;  d[4 i + 2 / 3] = the same columns 8 rows further.
+__device__ __forceinline__ void wgmma_m64n16k8_tf32(float d[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// one 32-float K chunk (4 instructions along K) of a 64 x (16 NB) accumulator: both operands K-major SWIZZLE_128B, the B rows 16 at a
+// time (16 rows x 128 B = 2048 bytes = 128 descriptor units).  NB is a compile-time constant, so the accumulators stay in registers.
+template <int NB, int NBMAX>
+__device__ __forceinline__ void mma_chunk(float (&acc)[NBMAX][8], uint64_t adesc, uint64_t bdesc, bool first) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int j = 0; j < NB; ++j)
+            wgmma_m64n16k8_tf32(acc[j], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(128 * j + 2 * k), (first && k == 0) ? 0u : 1u);
+}
+// the same with NB = nb chosen at run time among 1 .. NBMAX
+template <int NBMAX, int I = 1>
+__device__ __forceinline__ void mma_chunk_n(int nb, float (&acc)[NBMAX][8], uint64_t adesc, uint64_t bdesc, bool first) {
+    if constexpr (I <= NBMAX) {
+        if (nb == I) mma_chunk<I, NBMAX>(acc, adesc, bdesc, first);
+        else mma_chunk_n<NBMAX, I + 1>(nb, acc, adesc, bdesc, first);
+    }
 }
 
 }  // namespace cmgan_tc

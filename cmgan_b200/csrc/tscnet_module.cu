@@ -202,7 +202,7 @@ void dense_block(Run& r, float* cat, const std::string& p, int B, int T, int Fw,
 // 0.5 * FF(LN(x)) + x  (conformer.py:54-72,136-148,211-212)
 float* feed_forward(Run& r, const float* xin, long long M, const std::string& p) {
     float* out = r.alloc((size_t)M * C);
-    if (r.precision == 1) {          // fused kernel: hidden activation in TMEM / shared memory only (ffn_fused.cu)
+    if (r.precision == 1) {          // fused kernel: the hidden activation stays on the SM (ffn_fused.cu)
         float* w1p = r.alloc((size_t)4 * C * C);
         float* w2p = r.alloc((size_t)4 * C * C);
         if (r.live()) {
@@ -216,7 +216,7 @@ float* feed_forward(Run& r, const float* xin, long long M, const std::string& p)
     float* xn = r.alloc((size_t)M * C);
     float* stt = r.alloc((size_t)M * 2);
     float* a = r.alloc((size_t)M * 4 * C);
-    if (r.live()) r.ok(cmgan_ln_apply(xin, C, M, r.w(p + "fn.norm.weight"), r.w(p + "fn.norm.bias"), nullptr, 0, xn, C, stt, 0, r.st));
+    if (r.live()) r.ok(cmgan_ln_apply(xin, C, M, r.w(p + "fn.norm.weight"), r.w(p + "fn.norm.bias"), nullptr, 0, xn, C, stt, r.precision == 1 ? 1 : 0, r.st));
     Gemm g1(xn, C, r.w(p + "fn.fn.net.0.weight"), 0, 1, C, r.w(p + "fn.fn.net.0.bias"), nullptr, 4 * C, M, 4 * C, C);
     g1.a.epi = CMGAN_EPI_SWISH_DUAL; g1.a.C2 = a; g1.a.ldc2 = 4 * C;
     g1.run(r);

@@ -165,7 +165,7 @@ class TSCNet(nn.Module):
     def __init__(self, num_channel: int = 64, num_features: int = 201):
         super().__init__()
         if num_channel != C:
-            raise ValueError("the sm_100a kernels are specialised for num_channel=64 (the reference's only configuration)")
+            raise ValueError("the sm_90a kernels are specialised for num_channel=64 (the reference's only configuration)")
         self.num_channel, self.num_features = num_channel, num_features
         self._keys: List[str] = []
         for key, shape, kind, fan_in in _param_specs(num_channel, num_features):

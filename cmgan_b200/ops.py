@@ -21,15 +21,10 @@ SEED_DEV = None  # optional uint64 device counter added to every dropout seed (s
 WGRAD_STREAM = None   # optional side stream: weight-gradient GEMMs run there, concurrently with the data-gradient chain (join_wgrad)
 AUX_STREAM = None     # optional second side stream: the dk / dv half of the attention backward runs there, next to the dq / dE half
 _WGRAD_KEEP = []      # operands of in-flight side-stream launches (kept allocated until the join)
-# tf32 mode: attention forward on tcgen05 (csrc/attention_tc.cu) instead of mma.sync.  Off by default: the first tcgen05 version is
-# parity-green but 18 % slower than the mma.sync kernel (377 vs 318 us, B = 4 time axis; profiles/README.md), its softmax warps wait on a
-# serial S/R -> softmax -> PV chain with one TMEM slot per CTA.
-ATTN_TC = os.environ.get("CMGAN_ATTN_TC", "0") != "0"
 # attention backward: dE accumulators of the dq kernel in a block-private global scratch (60 KB of shared memory, 3 blocks / SM, any L) instead
 # of shared memory (110 KB at L = 321: 2 blocks / SM).  Off by default: measured equal at L = 321 (775 vs 773 us) and 5 % slower at L = 101
 # (300 vs 314 us) -- the kernel is not occupancy-bound; it is the variant to use when L > ~900, where the shared accumulator leaves 1 block / SM.
 ATTN_BWD_WS = os.environ.get("CMGAN_ATTN_BWD_WS", "0") != "0"
-FUSED_FFN = os.environ.get("CMGAN_FUSED_FFN", "1") != "0"   # tf32 mode: one tcgen05 kernel per feed-forward module (csrc/ffn_fused.cu)
 PACK_CACHE = None   # optional PackCache: re-tiled tensor-core weight operands kept across calls (owner refreshes them after every weight update)
 PROBE = None     # list collecting (entry point, M, N, K, start event, end event) when bench.py instruments a step
 
@@ -143,7 +138,7 @@ def join_wgrad() -> None:
 
 
 def set_precision(mode: str) -> None:
-    """'fp32' (exact FFMA) or 'tf32' (tcgen05 tensor cores for the dense contractions; fp32 storage, fp32 accumulate)"""
+    """'fp32' (exact FFMA) or 'tf32' (wgmma tensor cores for the dense contractions; fp32 storage, fp32 accumulate)"""
     global PRECISION
     assert mode in ("fp32", "tf32")
     PRECISION = 1 if mode == "tf32" else 0

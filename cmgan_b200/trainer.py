@@ -323,6 +323,13 @@ class FusedTrainer:
         self.static_clean, self.static_noisy = clean.clone(), noisy.clone()
         self._graph, self.static_loss = self._capture(lambda upd: self.generator_step(self.static_clean, self.static_noisy, update and upd, allreduce))
 
+    def release_graphs(self) -> None:
+        """drop the captured step graphs and the memory they hold (the next replay needs a new capture)"""
+        self._graph = self._tgraph = None
+        self.static_loss = self.static_losses = None
+        self.last = None
+        torch.cuda.empty_cache()
+
     def replay_generator_step(self, clean: torch.Tensor, noisy: torch.Tensor) -> torch.Tensor:
         self.static_clean.copy_(clean, non_blocking=True)
         self.static_noisy.copy_(noisy, non_blocking=True)

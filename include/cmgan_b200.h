@@ -1,4 +1,4 @@
-/* cmgan_b200 -- C ABI of the B200-native CMGAN hot path (libcmgan_b200.so).
+/* cmgan_b200 -- C ABI of the H100-native (sm_90a) CMGAN hot path (libcmgan_b200.so).
  *
  * The reference (ruizhecao96/CMGAN) has no FFI layer: its boundary for this path is the nn.Module
  * interface (TSCNet.forward generator.py:174-196, Discriminator.forward discriminator.py:62-64,
@@ -29,11 +29,11 @@ int cmgan_gemm_wgrad_f32(const CmganGemmArgs* a, void* stream);
 int cmgan_pack_weights(const CmganPackDesc* descs, int n, void* stream);
 int cmgan_pack_weight(const float* src, float* dst, long long sb_tap, long long sb_k, long long sb_n, int Cin, int ntaps, int N, void* stream);
 
-/* ---- fused macaron feed-forward (conformer.py:54-72,136-148,211-212): LN -> 64x256 -> Swish, dropout -> 256x64 -> dropout, alpha, residual in ONE tcgen05 kernel */
-int cmgan_ffn_fwd(const float* x, long long ldx, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1, const float* W2p, const float* b2, float alpha, unsigned long long seed1, unsigned long long seed2, unsigned int thr, float inv_keep, const unsigned long long* seed_dev, float* out, long long ldo, void* stream);
 
-int cmgan_ffn_debug_timeline(long long* buf);
-int cmgan_ffn_bwd(const float* x, long long ldx, const float* dz, long long lddz, const float* dout, long long lddo, const float* res2, long long ldr2, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1, const float* W2tp, const float* W1tp, unsigned long long seed1, unsigned int thr, float inv_keep, const unsigned long long* seed_dev, float* dx, long long lddx, float* a_out, float* dh_out, float* xn_out, float* dgamma, float* dbeta, void* stream);
+
+/* ---- fused macaron feed-forward (conformer.py:54-72,136-148,211-212): LN -> 64x256 -> Swish, dropout -> 256x64 -> dropout, alpha, residual in ONE wgmma kernel; backward recomputes the hidden layer (ws: M * 66 floats) */
+int cmgan_ffn_fwd(const float* x, long long ldx, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1, const float* W2p, const float* b2, float alpha, unsigned long long seed1, unsigned long long seed2, unsigned int thr, float inv_keep, const unsigned long long* seed_dev, float* out, long long ldo, void* stream);
+int cmgan_ffn_bwd(const float* x, long long ldx, const float* dz, long long lddz, const float* dout, long long lddo, const float* res2, long long ldr2, long long M, const float* ln_g, const float* ln_b, const float* W1p, const float* b1, const float* W2tp, const float* W1tp, unsigned long long seed1, unsigned int thr, float inv_keep, const unsigned long long* seed_dev, float* dx, long long lddx, float* a_out, float* dh_out, float* xn_out, float* dgamma, float* dbeta, float* ws, void* stream);
 
 /* ---- LayerNorm (conformer.py:68,161,214), InstanceNorm2d (generator.py:35,55,61,128,148), BatchNorm1d (conformer.py:169) */
 int cmgan_ln_stats(const float* x, long long ldx, long long M, float* stats, void* stream);
@@ -54,7 +54,6 @@ int cmgan_add_rows(const float* src, long long lds, float* dst, long long ldd, l
 int cmgan_attention_fwd(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, void* stream);
 int cmgan_attention_fwd_tf32(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, void* stream);
 int cmgan_attention_fwd_tf32_nbuf(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, int nbuf, void* stream);
-int cmgan_attention_fwd_tc(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, void* stream);
 int cmgan_attention_bwd(const float* qkv, const float* E, const float* ctx, const float* dctx, const float* lse, int B, int T, int F, int axis, float* delta, float* dqkv, float* dE, void* stream);
 int cmgan_attention_bwd_tf32_parts(const float* qkv, const float* E, const float* ctx, const float* dctx, const float* lse, int B, int T, int F, int axis, float* delta, float* dqkv, float* dE, int parts, void* stream);
 long long cmgan_attention_bwd_ws_floats(int B, int T, int F, int axis);

@@ -1,6 +1,6 @@
 """CPU oracle for the PESQ-free quality metrics of the reference's scoring tool -- TEST INFRASTRUCTURE ONLY.
 
-numpy restatement of ``snr`` (segmental SNR) and ``stoi`` of /root/reference/src/tools/compute_metrics.py, used by the parity
+numpy restatement of ``snr`` (segmental SNR) and ``stoi`` of the reference's src/tools/compute_metrics.py, used by the parity
 tests to report the SSNR / STOI deltas between this repo's enhanced waveforms and the reference's (SURVEY.md section 8c:
 PESQ itself is third-party C code, ``pesq==0.0.3``, absent from this image -- "parity unpinned" for PESQ only), and as the
 checker of the GPU scoring kernels (cmgan_b200.metrics).

@@ -1,4 +1,4 @@
-"""bench.py contract on the CPU: the reference arm (the reference's own modules when staged under baseline/_ref, else the oracle CPU
+"""bench.py contract on the CPU: the reference arm (the oracle CPU
 port) prints exactly one JSON line on stdout with the agreed keys."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Swish dual-output GEMM epilogue (feed-forward hidden layer): fp32 FFMA path vs float64, tf32 tcgen05 path vs fp32."""
+"""Swish dual-output GEMM epilogue (feed-forward hidden layer): fp32 FFMA path vs float64, tf32 wgmma path vs fp32."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""tcgen05 (tf32) GEMM path against the exact-fp32 FFMA path (itself checked against float64 in test_gpu_kernels.py)
+"""wgmma (tf32) GEMM path against the exact-fp32 FFMA path (itself checked against float64 in test_gpu_kernels.py)
 and end-to-end waveform parity in tf32 mode.  tf32 = 10 explicit mantissa bits: tolerance 4e-3 of the output range."""
 import os
 

@@ -1,5 +1,5 @@
 """The oracle (oracle/cmgan_oracle.py) against fixtures produced by the REFERENCE modules
-(tools/make_golden.py).  Runs everywhere (no /root/reference needed)."""
+(tools/make_golden.py).  Runs everywhere (no reference checkout needed)."""
 import numpy as np
 import torch
 

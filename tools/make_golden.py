@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/* from the REFERENCE implementation (run in the build container only).
 
-Imports the reference's own modules from /root/reference/src (generator.py, conformer.py,
+Imports the reference's own modules from $CMGAN_REFERENCE/src (a checkout of the original CMGAN repository) (generator.py, conformer.py,
 utils.py, discriminator.py with a stub ``pesq`` module) and the shipped checkpoint, runs them
 on CPU fp32 with fixed seeds and stores inputs + outputs as small .npz fixtures.  The glue of
 train.py / evaluation.py cannot be imported (module-level argparse, missing torchaudio/natsort,
@@ -17,7 +17,7 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/src"
+REF = os.path.join(os.environ.get("CMGAN_REFERENCE", "CMGAN"), "src")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 
@@ -201,7 +201,7 @@ def main():
 
     # ---- one real utterance from AudioSamples (first 1.0 s and the full 2.09 s file) -------
     from scipy.io import wavfile
-    sr, w = wavfile.read("/root/reference/AudioSamples/noisy/p232_170.wav")
+    sr, w = wavfile.read(os.path.join(REF, "..", "AudioSamples", "noisy", "p232_170.wav"))
     assert sr == 16000
     wavfile.write(os.path.join(OUT, "p232_170_noisy.wav"), sr, w)
     wf = torch.from_numpy(w.astype(np.float32) / 32768.0).unsqueeze(0)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/audiosamples.npz from the REFERENCE (run in the build container only).
 
-For each of the 25 utterances shipped under /root/reference/AudioSamples (2.1 .. 9.8 s, so the time-axis sequences reach
+For each of the 25 utterances shipped under $CMGAN_REFERENCE/AudioSamples (2.1 .. 9.8 s, so the time-axis sequences reach
 L = 1564 > 513: the relative-position clamp is exercised inside the whole network), this stores
   * the noisy and clean waveforms (int16, as shipped),
   * the reference's enhanced waveform: the reference's own TSCNet + power_compress/uncompress modules with the shipped
@@ -43,7 +43,7 @@ def main():
             log[m.group(1)] = (float(m.group(6)), float(m.group(7)))
     names, lens, noisy_all, clean_all, enh_all = [], [], [], [], []
     met = []
-    for f in sorted(glob.glob("/root/reference/AudioSamples/noisy/*.wav")):
+    for f in sorted(glob.glob(os.path.join(REF, "..", "AudioSamples", "noisy", "*.wav"))):
         name = os.path.basename(f)[:-4]
         sr, n16 = wavfile.read(f)
         sr2, c16 = wavfile.read(f.replace("/noisy/", "/clean/"))

@@ -12,7 +12,7 @@ import types
 
 import numpy as np
 
-REF = "/root/reference/src"
+REF = os.path.join(os.environ.get("CMGAN_REFERENCE", "CMGAN"), "src")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
