@@ -1,11 +1,18 @@
-// tf32 tensor-core weight gradient for sm_90a:  dW(tap, k, n) += sum_m pro(A[in_row(m, tap), k]) * prod(D[m, n])   (gemm_args.h, wgrad form)
+// tf32 tensor-core weight and bias gradient for sm_90a   (gemm_args.h, wgrad form)
+//     dW(tap, k, n) += sum_m pro(A[in_row(m, tap), k]) * prod(D[m, n])          dbias[n] += sum_m prod(D[m, n])
 //
-// The reduction runs over the rows m, while wgmma reads tf32 operands from shared memory only K-major, so both operands are transposed on
-// their way into shared memory: a stage holds 32 rows as A^T (64 k x 32 m) and D^T (N x 32 m), every line of 32 m-values one 128-byte
-// SWIZZLE_128B row.  One warpgroup per CTA: it stores the next stage (LDG, prologue / dropout scale applied, rounded to tf32) while the MMAs
-// of the current one run (wgmma m64n16k8, 4 K-steps per stage, N / 16 instructions per step), then adds its 64 x N tile into dW with
-// atomics (the parameter-gradient buffer is zeroed once per step).  Grid: (taps x k tiles, row chunks).  The bias gradient is a
-// separate column-sum pass.
+// The reduction runs over the rows m, and wgmma reads tf32 operands from shared memory only K-major, so both operands are transposed inside
+// the SM.  One CTA owns a 64 x Q tile of dW (Q <= 256) and a range of rows, which it streams in stages of 32 rows:
+//   - all 256 threads gather the stage's raw rows of A and D (row-major, as they lie in memory; convolution taps, strides and padding
+//     resolved per row) with 16-byte cp.async into a ring of 3 .. 6 slabs, so that several stages of loads are in flight at any time;
+//   - the same threads then read the oldest slab, apply the A prologue and D's dropout scale, add D into per-thread column sums for
+//     dbias, round to tf32 and write the K-major SWIZZLE_128B image (one 128-byte line of 32 m-values per k or n) that the descriptors read;
+//   - each warpgroup multiplies one half of the Q side of the image (m64n64k8 where Q allows, else m64n16k8) while the next image is
+//     being written into the other buffer.
+// The tile orientation is chosen per shape so that every CTA reads its rows of A and D once: either k on the wgmma M side and all N
+// columns on the Q side (P = A), or n on the M side and all Cin columns on the Q side (P = D, Cin <= 256).  At the end each CTA adds its
+// tile into dW (and, for one tile per tap-0 column range, its column sums into dbias) with atomics: the parameter-gradient buffer is
+// zeroed once per step.  The grid is as many CTAs as are resident at once (one wave).
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
 #include "gemm_device.cuh"
@@ -15,158 +22,301 @@ namespace {
 using namespace cmgan_gemm;
 using namespace cmgan_tc;
 
-constexpr int WT = 128;              // one warpgroup
+constexpr int NT = 256;              // two warpgroups
 constexpr int RS = 32;               // rows per stage = one 128-byte line of m-values
-constexpr int KT = 64;               // k values per tile = wgmma M
-constexpr int A_BYTES = KT * 128;    // 8 KB
+constexpr int PT = 64;               // lines on the P side = wgmma M
+constexpr int QMAX = 256;            // lines on the Q side, at most
+constexpr int MAX_RING = 6;
 
-// byte offset of (line, m) in a K-major SWIZZLE_128B tile of 32-float lines
-__device__ __forceinline__ uint32_t swz(int line, int m) { return (uint32_t)(line * 128 + ((((m >> 2) ^ line) & 7) << 4) + (m & 3) * 4); }
+struct Plan {
+    int ydir;              // 0: P = 64 k of A, Q = the N columns of D;  1: P = 64 n of D, Q = the Cin columns of A
+    int ptiles;            // 64-wide tiles along P per tap
+    int qpad;              // Q lines, rounded up to 32 (two warpgroups x a multiple of 16)
+    int wa, wd;            // raw row widths (floats) of the A and D slabs: multiples of 32
+    int ring;              // slabs in the cp.async ring
+    int mch;               // rows per CTA, a multiple of RS
+    uint32_t raw_bytes;    // one slab: A rows, D rows, in_row of each row (int), LN statistics of each row (float2)
+    uint32_t img_bytes;    // one operand image: P lines then Q lines, 128 bytes each
+};
 
-template <int NBMAX>
-__global__ void __launch_bounds__(WT) gemm_wgrad_tc_kernel(const __grid_constant__ CmganGemmArgs g, int mch) {
+// byte offset of 16-byte chunk c of row r in a raw slab of row width w floats.  The chunk index is XOR-swizzled by the row's m-group, so
+// that the eight lanes that read rows 4 g + i (g = 0..7) of one chunk hit eight different bank groups.
+__device__ __forceinline__ uint32_t raw_off(int r, int c, int w) { return (uint32_t)(r * w * 4 + ((c ^ ((r >> 2) & 7)) << 4)); }
+
+// one 32-row stage (4 K-steps of 8) of the warpgroup's 64 x 16 NB accumulator; `first` overwrites instead of accumulating
+template <int NB>
+__device__ __forceinline__ void mma_stage(float (&acc)[NB][8], uint64_t adesc, uint64_t bdesc, bool first) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
+        if constexpr (NB % 4 == 0) {
+#pragma unroll
+            for (int c = 0; c < NB / 4; ++c)
+                wgmma_m64n64k8_tf32(reinterpret_cast<float(&)[4][8]>(acc[4 * c]), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(512 * c + 2 * k),
+                                    accumulate);
+        } else {
+#pragma unroll
+            for (int j = 0; j < NB; ++j) wgmma_m64n16k8_tf32(acc[j], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(128 * j + 2 * k), accumulate);
+        }
+    }
+}
+__device__ __forceinline__ void cp_async_wait_n(int n) {
+    switch (n) {
+        case 0: cp_async_wait<0>(); break;
+        case 1: cp_async_wait<1>(); break;
+        case 2: cp_async_wait<2>(); break;
+        case 3: cp_async_wait<3>(); break;
+        default: cp_async_wait<4>(); break;
+    }
+}
+
+__device__ __forceinline__ float4 round4(float4 v) { return make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w)); }
+
+// NB = n16 accumulator blocks per warpgroup = qpad / 32.  Up to Q = 96 the shared memory holds two CTAs per SM, so the registers must too.
+template <int NB>
+__global__ void __launch_bounds__(NT, NB <= 3 ? 2 : 1) gemm_wgrad_tc_kernel(const __grid_constant__ CmganGemmArgs g, const Plan p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* const bptr = smem_raw + (base - smem_u32(smem_raw));
-    const int N = g.N, nb = N / 16;
-    const uint32_t stage_bytes = (uint32_t)(A_BYTES + N * 128);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ktiles = (g.Cin + KT - 1) / KT;
-    const int tap = blockIdx.x / ktiles, k0 = (blockIdx.x % ktiles) * KT;
-    const long mbeg = (long)blockIdx.y * mch;
-    const long mend = mbeg + mch < g.M ? mbeg + mch : g.M;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int tap = blockIdx.x / p.ptiles, p0 = (blockIdx.x % p.ptiles) * PT;
+    const int acol0 = p.ydir ? 0 : p0, na = p.ydir ? g.Cin : min(PT, g.Cin - p0);     // A columns of this tile
+    const int dcol0 = p.ydir ? p0 : 0, nd = p.ydir ? min(PT, g.N - p0) : g.N;        // D columns of this tile
+    const int la = p.ydir ? p.qpad : PT, ld = p.ydir ? PT : p.qpad;                   // image lines of A / D
+    const uint32_t aimg = p.ydir ? PT * 128 : 0, dimg = p.ydir ? 0 : PT * 128;        // their offsets inside an image
+    const long mbeg = (long)blockIdx.y * p.mch;
+    const long mend = mbeg + p.mch < g.M ? mbeg + p.mch : g.M;
+    const int nst = (int)((mend - mbeg + RS - 1) / RS);
+    if (nst <= 0) return;
     const unsigned long long seed = eff_seed(g);
-    // loader lanes: row m = (tid & 7) + 8 i, 4 consecutive columns (k or n) at 4 (tid >> 3) + 64 j -- 2-way bank conflicts on the transposed stores
-    const int lm = tid & 7, lq = (tid >> 3) * 4;
+    const bool do_bias = g.dbias != nullptr && tap == 0 && (p.ydir || p0 == 0);
+    uint8_t* const img0 = bptr;
+    uint8_t* const ring = bptr + 2 * p.img_bytes;
+    const uint32_t dslab = (uint32_t)(RS * p.wa * 4), rows_off = (uint32_t)(RS * (p.wa + p.wd) * 4), stats_off = rows_off + RS * 4;
 
-    auto load_stage = [&](long mb, int buf) {
-        uint8_t* sa = bptr + buf * stage_bytes;
-        uint8_t* sd = sa + A_BYTES;
+    // stage s -> slab `slot`: thread t gathers row t / 8 of the stage, 16-byte chunks t % 8, t % 8 + 8, ... of its A and D columns
+    auto issue = [&](int s, int slot) {
+        uint8_t* const sl = ring + slot * p.raw_bytes;
+        const int row = tid >> 3, c8 = tid & 7;
+        const long m = mbeg + (long)s * RS + row;
+        long r = -1;
+        if (m < mend) r = in_row_of(g, decode_row(g, (int)m), tap);
+        if (c8 == 0) reinterpret_cast<int*>(sl + rows_off)[row] = (int)r;
+        if (r >= 0) {
+            const float* src = g.A + g.tap_off[tap] + r * g.lda + acol0;
+            for (int c = c8; c < na / 4; c += 8) cp_async16(smem_u32(sl + raw_off(row, c, p.wa)), src + 4 * c, 16);
+            if (g.pro == CMGAN_PRO_LN && c8 == 0) cp_async8(smem_u32(sl + stats_off + row * 8), g.p0 + 2 * r);
+        }
+        if (m < mend) {
+            const float* src = g.D + m * g.ldd + dcol0;
+            for (int c = c8; c < nd / 4; c += 8) cp_async16(smem_u32(sl + dslab + raw_off(row, c, p.wd)), src + 4 * c, 16);
+        }
+    };
+
+    // item it < 2 ld: D lines 4 lb .. 4 lb + 3 x rows 4 q .. 4 q + 3 (lb = it / 8, q = it % 8); then the same for A.  A thread keeps its
+    // D items from stage to stage, so it keeps their column sums in registers (at most 2 items: ld <= 256).
+    float cs[2][4] = {};
+    auto colsum = [](float (&c)[4], const float4 (&v)[4]) {
 #pragma unroll
-        for (int i = 0; i < RS / 8; ++i) {
-            const int ml = lm + 8 * i;
-            const long m = mb + ml;
-            RowInfo ri = decode_row(g, (int)(m < mend ? m : g.M));
-            if (m >= mend) ri.ok = false;
-            float a[4];
-            load_a4<4>(g, in_row_of(g, ri, tap), tap, k0 + lq, a);
+        for (int i = 0; i < 4; ++i) { c[0] += v[i].x; c[1] += v[i].y; c[2] += v[i].z; c[3] += v[i].w; }
+    };
+    auto transform = [&](int s, int slot, uint8_t* img) {
+        const uint8_t* const sl = ring + slot * p.raw_bytes;
+        const int* const rows = reinterpret_cast<const int*>(sl + rows_off);
+        const float2* const stats = reinterpret_cast<const float2*>(sl + stats_off);
+        const long mb = mbeg + (long)s * RS;
+#pragma unroll 1
+        for (int u = 0; u < 3; ++u) {
+            const int it = tid + u * NT;
+            if (it >= 2 * (ld + la)) break;
+            const bool isd = it < 2 * ld;
+            const int j = isd ? it : it - 2 * ld, lb = j >> 3, q = j & 7;
+            float4 v[4];
+            if (4 * lb < (isd ? nd : na)) {
+                const uint8_t* const src = isd ? sl + dslab : sl;
+                const int w = isd ? p.wd : p.wa;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) *reinterpret_cast<float*>(sa + swz(lq + j, ml)) = to_tf32(a[j]);
-            for (int n = lq; n < N; n += 64) {
-                float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (m < mend) d = __ldg(reinterpret_cast<const float4*>(g.D + m * g.ldd + n));
-                float dv[4] = {d.x, d.y, d.z, d.w};
+                for (int i = 0; i < 4; ++i) v[i] = *reinterpret_cast<const float4*>(src + raw_off(4 * q + i, lb, w));
+                if (isd) {
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    if (g.prod == 1 && m < mend) dv[j] *= g.alpha * cmgan_drop_scale(seed, (uint64_t)m * N + n + j, g.drop_thr, g.inv_keep);
-                    *reinterpret_cast<float*>(sd + swz(n + j, ml)) = to_tf32(dv[j]);
+                    for (int i = 0; i < 4; ++i) {
+                        const long m = mb + 4 * q + i;
+                        if (m >= mend) { v[i] = make_float4(0.f, 0.f, 0.f, 0.f); continue; }
+                        if (g.prod == 1) {
+                            float ds[4];
+                            cmgan_drop_scale4(seed, (uint64_t)m * g.N + dcol0 + 4 * lb, g.drop_thr, g.inv_keep, ds);
+                            v[i].x *= g.alpha * ds[0]; v[i].y *= g.alpha * ds[1]; v[i].z *= g.alpha * ds[2]; v[i].w *= g.alpha * ds[3];
+                        }
+                    }
+                    if (do_bias) {
+                        if (u == 0) colsum(cs[0], v);
+                        else colsum(cs[1], v);
+                    }
+                } else {
+                    const int k = acol0 + 4 * lb;
+                    ChunkParams cp;
+                    load_chunk_params(g, k, cp);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int r = rows[4 * q + i];
+                        if (r < 0) { v[i] = make_float4(0.f, 0.f, 0.f, 0.f); continue; }
+                        if (g.pro != CMGAN_PRO_NONE) {
+                            const float2 st = g.pro == CMGAN_PRO_LN ? stats[4 * q + i] : make_float2(0.f, 0.f);
+                            v[i] = transform4(g, v[i], r, k, st.x, st.y, cp);
+                        }
+                    }
                 }
+            } else {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[i] = round4(v[i]);
+            // line L = 4 lb + e of the image holds (v[0].e, v[1].e, v[2].e, v[3].e) at m-group q
+            uint8_t* const dst = img + (isd ? dimg : aimg);
+            const int L = 4 * lb;
+            *reinterpret_cast<float4*>(dst + (L + 0) * 128 + (((q ^ (L + 0)) & 7) << 4)) = make_float4(v[0].x, v[1].x, v[2].x, v[3].x);
+            *reinterpret_cast<float4*>(dst + (L + 1) * 128 + (((q ^ (L + 1)) & 7) << 4)) = make_float4(v[0].y, v[1].y, v[2].y, v[3].y);
+            *reinterpret_cast<float4*>(dst + (L + 2) * 128 + (((q ^ (L + 2)) & 7) << 4)) = make_float4(v[0].z, v[1].z, v[2].z, v[3].z);
+            *reinterpret_cast<float4*>(dst + (L + 3) * 128 + (((q ^ (L + 3)) & 7) << 4)) = make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
         }
         fence_proxy_async();          // generic-proxy stores -> visible to the tensor core's async proxy
     };
 
-    float acc[NBMAX][8];
-#pragma unroll
-    for (int j = 0; j < NBMAX; ++j)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[j][i] = 0.f;
-    const int nst = (int)((mend - mbeg + RS - 1) / RS);
-    if (nst > 0) load_stage(mbeg, 0);
-    __syncthreads();
-    for (int st = 0; st < nst; ++st) {
-        const uint32_t sa = base + (st & 1) * stage_bytes;
-        wgmma_fence();
-        mma_chunk_n<NBMAX>(nb, acc, gmma_desc_sw128(sa), gmma_desc_sw128(sa + A_BYTES), st == 0);
-        wgmma_commit();
-        if (st + 1 < nst) load_stage(mbeg + (long)(st + 1) * RS, (st + 1) & 1);     // the other buffer: its MMAs retired last iteration
-        wgmma_wait<0>();
-        __syncthreads();
+    float acc[NB][8];      // written first by the MMAs of stage 0 (nst >= 1)
+    const int qh = NB * 16;
+
+    // one commit group per stage (empty past the end), so that "stage s has landed" is always "at most ring - 2 groups pending"
+    for (int s = 0; s < p.ring - 1; ++s) {
+        if (s < nst) issue(s, s);
+        cp_async_commit();
     }
-    if (nst == 0) return;
-    // fragment of warp w: k = k0 + 16 w + lane / 4 (+ 8), n = 16 j + 8 i + 2 (lane % 4) (+ 1)
-    const int kr = k0 + 16 * warp + (lane >> 2), nc = 2 * (lane & 3);
+    for (int s = 0; s < nst; ++s) {
+        cp_async_wait_n(p.ring - 2);
+        __syncthreads();              // stage s visible to all; the slab and image of stage s - 2 / s - 1 are no longer read
+        if (s + p.ring - 1 < nst) issue(s + p.ring - 1, (s + p.ring - 1) % p.ring);
+        cp_async_commit();
+        uint8_t* const img = img0 + (s & 1) * p.img_bytes;
+        transform(s, s % p.ring, img);
+        __syncthreads();
+        const uint32_t ia = smem_u32(img);
+        wgmma_fence();
+        mma_stage<NB>(acc, gmma_desc_sw128(ia), gmma_desc_sw128(ia + PT * 128 + wg * qh * 128), s == 0);
+        wgmma_commit();
+        wgmma_wait<1>();              // the MMAs of stage s - 1 are done: its image buffer is written next
+    }
+    wgmma_wait<0>();
+
+    // fragment of warp w of warpgroup h: P line 16 (w % 4) + lane / 4 (+ 8), Q line h qh + 16 j + 8 i + 2 (lane % 4) (+ 1)
+    const int pl = 16 * (warp & 3) + (lane >> 2), ql = wg * qh + 2 * (lane & 3);
     float* const dst = g.C + (long)tap * g.sb_tap;
 #pragma unroll
-    for (int j = 0; j < NBMAX; ++j) {
-        if (j >= nb) break;
+    for (int j = 0; j < NB; ++j) {
 #pragma unroll
-        for (int i = 0; i < 2; ++i)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int k = kr + 8 * h;
-                if (k >= g.Cin) continue;
-                const int n = 16 * j + 8 * i + nc;
-                atomicAdd(dst + (long)k * g.sb_k + (long)n * g.sb_n, acc[j][4 * i + 2 * h]);
-                atomicAdd(dst + (long)k * g.sb_k + (long)(n + 1) * g.sb_n, acc[j][4 * i + 2 * h + 1]);
-            }
-    }
-}
-
-// dbias[n] += sum_m prod(D[m, n])
-__global__ void colsum_kernel(const float* __restrict__ D, long ldd, long M, int N, int prod, float alpha, unsigned long long seed, unsigned thr,
-                              float inv_keep, int rows_per_block, float* __restrict__ out, const unsigned long long* __restrict__ seed_dev) {
-    seed = cmgan_eff_seed(seed, seed_dev);
-    __shared__ float sm[256];
-    const int c = threadIdx.x % N, rg = threadIdx.x / N, nrg = blockDim.x / N;
-    const long r_beg = (long)blockIdx.x * rows_per_block;
-    const long r_end = r_beg + rows_per_block < M ? r_beg + rows_per_block : M;
-    float s = 0.f;
-    if (rg < nrg)
-        for (long m = r_beg + rg; m < r_end; m += nrg) {
-            float d = __ldg(D + m * ldd + c);
-            if (prod == 1) d *= alpha * cmgan_drop_scale(seed, (uint64_t)m * N + c, thr, inv_keep);
-            s += d;
+        for (int e = 0; e < 8; ++e) {
+            const int pe = p0 + pl + 8 * ((e >> 1) & 1), qe = ql + 16 * j + 8 * (e >> 2) + (e & 1);
+            const int k = p.ydir ? qe : pe, n = p.ydir ? pe : qe;
+            if (k < g.Cin && n < g.N) atomicAdd(dst + (long)k * g.sb_k + (long)n * g.sb_n, acc[j][e]);
         }
-    sm[threadIdx.x] = s;
-    __syncthreads();
-    if (threadIdx.x < N) {
-        float t = 0.f;
-        for (int q = 0; q < nrg; ++q) t += sm[q * N + c];
-        atomicAdd(out + c, t);
+    }
+    if (do_bias) {
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int it = tid + u * NT;
+            if (it >= 2 * ld) break;                    // uniform per warp: 2 ld is a multiple of 64
+            const int lb = it >> 3;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float v = cs[u][e];
+                v += __shfl_xor_sync(0xffffffffu, v, 1);
+                v += __shfl_xor_sync(0xffffffffu, v, 2);
+                v += __shfl_xor_sync(0xffffffffu, v, 4);
+                if ((it & 7) == 0 && 4 * lb + e < nd) atomicAdd(g.dbias + dcol0 + 4 * lb + e, v);
+            }
+        }
     }
 }
 
 int wgrad_tc_supported(const CmganGemmArgs* a) {
-    if (a->N % 16 || a->N < 16 || a->N > 256) return 0;
+    if (a->N % 16 || a->N < 16 || a->N > QMAX) return 0;
     if (a->Cin % 4 || a->lda % 4 || ((uintptr_t)a->A & 15) || a->ldd % 4 || ((uintptr_t)a->D & 15)) return 0;
     for (int t = 0; t < a->ntaps; ++t)
         if (a->tap_off[t] % 4) return 0;
     return 1;
 }
 
-template <int NBMAX>
-int launch(const CmganGemmArgs* a, dim3 grid, size_t smem, int mch, cudaStream_t st) {
+// shared memory of an SM and the opt-in limit of one CTA (queried once)
+int smem_limits(int* per_sm, int* per_block) {
+    static int sm = 0, blk = 0;
+    if (!sm) {
+        int dev = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&blk, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        if (e != cudaSuccess) { sm = 0; cmgan_set_error("gemm_wgrad_tc: device attributes: %s", cudaGetErrorString(e)); return -1; }
+    }
+    *per_sm = sm;
+    *per_block = blk;
+    return 0;
+}
+
+template <int NB>
+int launch(const CmganGemmArgs* a, Plan p, size_t smem, int smem_blk, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_tc_kernel<NBMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 1024));
+        cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_tc_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_blk);
         if (e != cudaSuccess) { cmgan_set_error("gemm_wgrad_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
         attr_set = true;
     }
-    gemm_wgrad_tc_kernel<NBMAX><<<grid, WT, smem, st>>>(*a, mch);
+    int occ = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gemm_wgrad_tc_kernel<NB>, NT, smem);
+    if (e != cudaSuccess || occ < 1) { cmgan_set_error("gemm_wgrad_tc: occupancy query: %s (%d CTAs)", cudaGetErrorString(e), occ); return -1; }
+    // one wave: the resident CTAs split the rows evenly between them
+    const long tiles = (long)a->ntaps * p.ptiles;
+    long chunks = ((long)occ * cmgan_num_sms()) / tiles;
+    if (chunks < 1) chunks = 1;
+    const long max_chunks = (a->M + RS - 1) / RS;
+    if (chunks > max_chunks) chunks = max_chunks;
+    const long mch = (a->M + chunks - 1) / chunks;
+    p.mch = (int)(((mch + RS - 1) / RS) * RS);
+    const dim3 grid((unsigned)tiles, (unsigned)((a->M + p.mch - 1) / p.mch));
+    gemm_wgrad_tc_kernel<NB><<<grid, NT, smem, st>>>(*a, p);
     return cmgan_check_launch("gemm_wgrad_tc_kernel");
 }
 
 }  // namespace
 
-// tf32 tensor-core path of cmgan_gemm_wgrad (same contract).  Returns 1 if the shape is not covered (caller runs the fp32 kernels).
+// tf32 tensor-core path of cmgan_gemm_wgrad (same contract, bias gradient included).  Returns 1 if the shape is not covered (the caller
+// runs the fp32 kernels).
 int cmgan_gemm_wgrad_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
     if (!wgrad_tc_supported(a)) return 1;
-    const int ytiles = ((a->Cin + KT - 1) / KT) * a->ntaps;
-    // rows per CTA: about four resident CTAs per SM in one wave (every CTA ends with one atomic pass over its dW tile), at least 8 stages
-    long want = (4L * cmgan_num_sms()) / ytiles;
-    if (want < 1) want = 1;
-    long mch = (a->M + want - 1) / want;
-    mch = ((mch + RS - 1) / RS) * RS;
-    if (mch < 8 * RS) mch = 8 * RS;
-    const dim3 grid((unsigned)ytiles, (unsigned)((a->M + mch - 1) / mch));
-    const size_t smem = 1024 + 2 * (size_t)(A_BYTES + a->N * 128);
-    const int rc = a->N <= 64 ? launch<4>(a, grid, smem, (int)mch, st) : launch<16>(a, grid, smem, (int)mch, st);
-    if (rc) return rc;
-    if (a->dbias) {
-        const int rpb = 64 * (256 / a->N > 0 ? 256 / a->N : 1);     // ~64 rows per thread -> thousands of blocks
-        colsum_kernel<<<cdiv(a->M, rpb), 256, 0, st>>>(a->D, a->ldd, a->M, a->N, a->prod, a->alpha, a->seed, a->drop_thr, a->inv_keep, rpb, a->dbias, a->seed_dev);
-        return cmgan_check_launch("colsum_kernel");
+    if (a->M <= 0) return 0;
+    int smem_sm, smem_blk;
+    if (smem_limits(&smem_sm, &smem_blk)) return -1;
+    Plan p{};
+    // orientation: the one that reads fewer bytes of A and D in total (every tile reads all rows of its columns)
+    const long cost_x = (long)cdiv(a->Cin, PT) * (PT + a->N), cost_y = (long)cdiv(a->N, PT) * (a->Cin + PT);
+    p.ydir = a->Cin <= QMAX && cost_y < cost_x;
+    p.ptiles = p.ydir ? cdiv(a->N, PT) : cdiv(a->Cin, PT);
+    p.qpad = (((p.ydir ? a->Cin : a->N) + 31) / 32) * 32;
+    p.wa = p.ydir ? p.qpad : PT;
+    p.wd = p.ydir ? PT : p.qpad;
+    p.raw_bytes = (uint32_t)(RS * (p.wa + p.wd) * 4 + RS * 4 + RS * 8);
+    p.img_bytes = (uint32_t)((PT + p.qpad) * 128);
+    // two CTAs per SM when a ring of at least 3 slabs fits in half the shared memory, else one CTA with a deeper ring
+    long ring = (smem_sm / 2 - 2048 - 2L * p.img_bytes) / p.raw_bytes;     // per-CTA reservation + alignment slack + the two images
+    if (ring < 3) ring = (smem_blk - 1024 - 2L * p.img_bytes) / p.raw_bytes;
+    if (ring < 3) { cmgan_set_error("gemm_wgrad_tc: %d x %d tile does not fit in shared memory", PT, p.qpad); return -1; }
+    p.ring = ring > MAX_RING ? MAX_RING : (int)ring;
+    const size_t smem = 1024 + 2 * (size_t)p.img_bytes + (size_t)p.ring * p.raw_bytes;
+    switch (p.qpad / 32) {
+        case 1: return launch<1>(a, p, smem, smem_blk, st);
+        case 2: return launch<2>(a, p, smem, smem_blk, st);
+        case 3: return launch<3>(a, p, smem, smem_blk, st);
+        case 4: return launch<4>(a, p, smem, smem_blk, st);
+        case 5: return launch<5>(a, p, smem, smem_blk, st);
+        case 6: return launch<6>(a, p, smem, smem_blk, st);
+        case 7: return launch<7>(a, p, smem, smem_blk, st);
+        default: return launch<8>(a, p, smem, smem_blk, st);
     }
-    return 0;
 }

@@ -54,6 +54,9 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const void* tmap,
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
 }
+__device__ __forceinline__ void cp_async8(uint32_t dst_smem, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst_smem), "l"(src) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -87,6 +90,17 @@ __device__ __forceinline__ void wgmma_m64n16k8_tf32(float d[8], uint64_t adesc, 
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                  : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// D[64 x 64] (+)= A[64 x 8] B[64 x 8]^T: the fragment of d[b] (b = 0..3) is that of the m64n16k8 instruction on columns 16 b .. 16 b + 15
+#define CMGAN_D8(b) "+f"(d[b][0]), "+f"(d[b][1]), "+f"(d[b][2]), "+f"(d[b][3]), "+f"(d[b][4]), "+f"(d[b][5]), "+f"(d[b][6]), "+f"(d[b][7])
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[4][8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 : CMGAN_D8(0), CMGAN_D8(1), CMGAN_D8(2), CMGAN_D8(3)
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+#undef CMGAN_D8
 
 // one 32-float K chunk (4 instructions along K) of a 64 x (16 NB) accumulator: both operands K-major SWIZZLE_128B, the B rows 16 at a
 // time (16 rows x 128 B = 2048 bytes = 128 descriptor units).  NB is a compile-time constant, so the accumulators stay in registers.

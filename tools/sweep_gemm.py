@@ -66,14 +66,14 @@ report("rows N=256 K=64 PRO_LN", timeit(lambda: gemm(A=x64, lda=64, W=W[(256, 64
 # wgrads
 dw = torch.zeros(256, 64, device=dev)
 db = torch.zeros(256, device=dev)
-report("wgrad N=256 K=64 (+colsum)", timeit(lambda: gemm(wgrad=True, W=None, C=dw, ldc=0, dbias=db, A=x64, lda=64, Cin=64, D=x256, ldd=256, N=256, sb_k=1,
+report("wgrad N=256 K=64 (+dbias)", timeit(lambda: gemm(wgrad=True, W=None, C=dw, ldc=0, dbias=db, A=x64, lda=64, Cin=64, D=x256, ldd=256, N=256, sb_k=1,
                                                       sb_n=64, M=M)), M * (64 + 256) * F4)
 report("wgrad N=256 K=64 (no dbias)", timeit(lambda: gemm(wgrad=True, W=None, C=dw, ldc=0, A=x64, lda=64, Cin=64, D=x256, ldd=256, N=256, sb_k=1,
                                                        sb_n=64, M=M)), M * (64 + 256) * F4)
 dw2 = torch.zeros(64, 256, device=dev)
 db2 = torch.zeros(64, device=dev)
-report("wgrad N=64 K=256 (+colsum)", timeit(lambda: gemm(wgrad=True, W=None, C=dw2, ldc=0, dbias=db2, A=x256, lda=256, Cin=256, D=x64, ldd=64, N=64, sb_k=1,
+report("wgrad N=64 K=256 (+dbias)", timeit(lambda: gemm(wgrad=True, W=None, C=dw2, ldc=0, dbias=db2, A=x256, lda=256, Cin=256, D=x64, ldd=64, N=64, sb_k=1,
                                                       sb_n=256, M=M)), M * (64 + 256) * F4)
 dw3 = torch.zeros(64, 64, device=dev)
-report("wgrad N=64 K=64 (+colsum)", timeit(lambda: gemm(wgrad=True, W=None, C=dw3, ldc=0, dbias=db2, A=x64, lda=64, Cin=64, D=r64, ldd=64, N=64, sb_k=1,
+report("wgrad N=64 K=64 (+dbias)", timeit(lambda: gemm(wgrad=True, W=None, C=dw3, ldc=0, dbias=db2, A=x64, lda=64, Cin=64, D=r64, ldd=64, N=64, sb_k=1,
                                                      sb_n=64, M=M)), M * (64 + 64) * F4)
