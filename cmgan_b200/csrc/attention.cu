@@ -66,13 +66,17 @@ __device__ __forceinline__ void stage_E(float* dst, const float* E, int rfirst, 
 }
 
 // ------------------------------------------------------------------------------------------ forward
+// RAGGED: sequence s has its own length (ragged_seq_len); blocks past it exit, keys past it are never staged
+template <bool RAGGED>
 __global__ void __launch_bounds__(NTH) attn_fwd_kernel(const float* __restrict__ qkv, SeqGeom g, const float* __restrict__ E,
-                                                       float* __restrict__ ctx, float* __restrict__ lse) {
+                                                       float* __restrict__ ctx, float* __restrict__ lse, const int* __restrict__ tlen, int axis) {
     __shared__ __align__(16) float Ks[TILE * D], Vs[TILE * D], Es[WROWS * WLD];
     const int s = blockIdx.x / H, h = blockIdx.x % H;
     const int i0 = blockIdx.y * NTH, il = threadIdx.x, i = i0 + il;
+    const int L = RAGGED ? ragged_seq_len(g, s, tlen, axis) : g.L;
+    if (RAGGED && i0 >= L) return;
     const long base = seq_base(g, s);
-    const bool active = i < g.L;
+    const bool active = i < L;
     float q[D], acc[D];
 #pragma unroll
     for (int d = 0; d < D; ++d) { q[d] = 0.f; acc[d] = 0.f; }
@@ -82,11 +86,11 @@ __global__ void __launch_bounds__(NTH) attn_fwd_kernel(const float* __restrict__
         for (int d = 0; d < D; ++d) q[d] *= SCALE_LOG2E;
     }
     float mrun = -INFINITY, lrun = 0.f;
-    for (int j0 = 0; j0 < g.L; j0 += TILE) {
-        const int nk = min(TILE, g.L - j0);
+    for (int j0 = 0; j0 < L; j0 += TILE) {
+        const int nk = min(TILE, L - j0);
         __syncthreads();
-        stage_rows16(Ks, qkv + CQ + h * D, base, g.tok_stride, j0, nk, g.L, 1.f);
-        stage_rows16(Vs, qkv + 2 * CQ + h * D, base, g.tok_stride, j0, nk, g.L, 1.f);
+        stage_rows16(Ks, qkv + CQ + h * D, base, g.tok_stride, j0, nk, L, 1.f);
+        stage_rows16(Vs, qkv + 2 * CQ + h * D, base, g.tok_stride, j0, nk, L, 1.f);
         // r = i - j = (i0 - j0) + (il - jl);  window row w = il - jl + TILE - 1
         stage_E(Es, E, i0 - j0 - (TILE - 1), NTH + nk - 1 + (TILE - nk));
         __syncthreads();
@@ -360,7 +364,19 @@ CMGAN_API int cmgan_attention_fwd(const float* qkv, const float* E, int B, int T
     SeqGeom g = geom_from(B, T, F, axis);
     if (g.n_seq == 0 || g.L == 0) return 0;
     dim3 grid(g.n_seq * H, cdiv(g.L, NTH));
-    attn_fwd_kernel<<<grid, NTH, 0, (cudaStream_t)stream>>>(qkv, g, E, ctx, lse);
+    attn_fwd_kernel<false><<<grid, NTH, 0, (cudaStream_t)stream>>>(qkv, g, E, ctx, lse, nullptr, axis);
+    return cmgan_check_launch("attn_fwd_kernel");
+}
+
+// ragged batch: utterance b has frames[b] valid frames (frames t >= T_b of qkv are never read; ctx / lse rows there are left unwritten)
+CMGAN_API int cmgan_attention_fwd_ragged(const float* qkv, const float* E, int B, int T, int F, int axis, const int* frames, float* ctx, float* lse,
+                                         void* stream) {
+    CMGAN_REQUIRE(qkv && E && ctx && frames, "cmgan_attention_fwd_ragged: null pointer");
+    CMGAN_REQUIRE(axis == 0 || axis == 1, "cmgan_attention_fwd_ragged: axis must be 0 (time) or 1 (freq)");
+    SeqGeom g = geom_from(B, T, F, axis);
+    if (g.n_seq == 0 || g.L == 0) return 0;
+    dim3 grid(g.n_seq * H, cdiv(g.L, NTH));
+    attn_fwd_kernel<true><<<grid, NTH, 0, (cudaStream_t)stream>>>(qkv, g, E, ctx, lse, frames, axis);
     return cmgan_check_launch("attn_fwd_kernel");
 }
 

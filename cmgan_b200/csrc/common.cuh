@@ -113,6 +113,14 @@ struct SeqGeom {
 __host__ __device__ __forceinline__ long seq_base(const SeqGeom& g, int s) {
     return (long)(s / g.n_inner) * g.outer_stride + (long)(s % g.n_inner) * g.inner_stride;
 }
+// Ragged batches: utterance b holds tlen[b] valid frames t < T_b of the (B, T, F) grid; frames t >= T_b are don't-care and are never read.
+// Valid length of sequence s: time axis -> T_b (clamped to [0, T]); frequency axis -> F for a frame t < T_b, else 0 (the sequence is skipped).
+__device__ __forceinline__ int clamp_len(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
+__device__ __forceinline__ int ragged_seq_len(const SeqGeom& g, int s, const int* __restrict__ tlen, int axis) {
+    const int b = s / g.n_inner;
+    if (axis == 0) return clamp_len(__ldg(tlen + b), g.L);
+    return (s % g.n_inner) < clamp_len(__ldg(tlen + b), g.n_inner) ? g.L : 0;
+}
 static inline SeqGeom make_seq_geom(int B, int T, int F, int axis /*0 = time, 1 = freq*/) {
     SeqGeom g;
     if (axis == 0) { g.n_seq = B * F; g.L = T; g.n_inner = F; g.outer_stride = (long)T * F; g.inner_stride = 1; g.tok_stride = F; }

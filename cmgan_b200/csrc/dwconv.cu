@@ -60,9 +60,19 @@ __device__ __forceinline__ void store_chunk(const ChunkRegs& r, float* U, float*
 
 // forward.  bn_sums (optional): per-channel sum / sum of squares of the output (sums[c * 2 + {0, 1}], BatchNorm1d batch statistics,
 // conformer.py:169) accumulated here instead of by a separate pass over `out`.
+//
+// RAGGED (inference): utterance b has tlen[b] valid frames.  The flattened space holds only valid tiles: utterance b contributes
+// (time axis) F sequences of length T_b or (frequency axis) T_b sequences of length F, and a prefix over the nb utterances maps a tile to
+// its sequence.  Rows past a sequence's own end read as zeros, the padding Conv1d(padding = 15) gives an utterance run alone.
+__device__ __forceinline__ long ragged_tiles(const SeqGeom& sg, const int* __restrict__ tlen, int b, int axis) {
+    if (axis == 0) return (long)sg.n_inner * ((clamp_len(__ldg(tlen + b), sg.L) + CK - 1) / CK);
+    return (long)clamp_len(__ldg(tlen + b), sg.n_inner) * ((sg.L + CK - 1) / CK);
+}
+
+template <bool RAGGED>
 __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __restrict__ g, SeqGeom sg, const float* __restrict__ w,
                                                                 const float* __restrict__ bias, float* __restrict__ out,
-                                                                double* __restrict__ bn_sums) {
+                                                                double* __restrict__ bn_sums, const int* __restrict__ tlen, int nb, int axis) {
     __shared__ __align__(16) float U[RING * CH];
     const int c = threadIdx.x & (CH - 1), half = threadIdx.x >> 7;
     float wr[KS];
@@ -70,25 +80,44 @@ __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __r
     for (int k = 0; k < KS; ++k) wr[k] = __ldg(w + c * KS + k);
     const float bs = __ldg(bias + c);
     float s1 = 0.f, s2 = 0.f;
-    const int tps = (sg.L + CK - 1) / CK;
-    const long total = (long)sg.n_seq * tps;
+    int L = sg.L, tps = (sg.L + CK - 1) / CK;
+    long total = (long)sg.n_seq * tps;
+    if (RAGGED) {
+        total = 0;
+        for (int b = 0; b < nb; ++b) total += ragged_tiles(sg, tlen, b, axis);
+    }
     long tile = total * blockIdx.x / gridDim.x;
     const long hi = total * (blockIdx.x + 1) / gridDim.x;
     ChunkRegs regs;
     while (tile < hi) {
-        const int s = (int)(tile / tps), k0 = (int)(tile % tps);
+        int s, k0;
+        if (RAGGED) {
+            long rem = tile;
+            int b = 0;
+            for (; b < nb - 1; ++b) {
+                const long n = ragged_tiles(sg, tlen, b, axis);
+                if (rem < n) break;
+                rem -= n;
+            }
+            if (axis == 0) { L = clamp_len(__ldg(tlen + b), sg.L); tps = (L + CK - 1) / CK; }
+            s = b * sg.n_inner + (int)(rem / tps);
+            k0 = (int)(rem % tps);
+        } else {
+            s = (int)(tile / tps);
+            k0 = (int)(tile % tps);
+        }
         const int kend = (int)min((long)tps, k0 + (hi - tile));
         const long base = seq_base(sg, s);
         __syncthreads();                                        // the previous run is done with the ring
 #pragma unroll 1
         for (int ch = k0 - 1; ch <= k0 + 1; ++ch) {
-            load_chunk<false>(regs, g, nullptr, base, sg.tok_stride, ch, sg.L);
+            load_chunk<false>(regs, g, nullptr, base, sg.tok_stride, ch, L);
             store_chunk<false>(regs, U, nullptr, nullptr, ch);
         }
         __syncthreads();
 #pragma unroll 1
         for (int k = k0; k < kend; ++k) {
-            load_chunk<false>(regs, g, nullptr, base, sg.tok_stride, k + 2, sg.L);
+            load_chunk<false>(regs, g, nullptr, base, sg.tok_stride, k + 2, L);
             const int tok0 = k * CK + half * TOK;
             const int rs = (tok0 - PADL) & (RING - 1), wm = RING - rs;          // sweep row m lives at ring row (rs + m) mod 64
             const float* p1 = U + rs * CH + c;
@@ -106,7 +135,7 @@ __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __r
 #pragma unroll
             for (int i = 0; i < TOK; ++i) {
                 const int tok = tok0 + i;
-                if (tok < sg.L) {
+                if (tok < L) {
                     out[(base + (long)tok * sg.tok_stride) * CH + c] = acc[i];
                     s1 += acc[i];
                     s2 = fmaf(acc[i], acc[i], s2);
@@ -232,7 +261,20 @@ CMGAN_API int cmgan_glu_dwconv_fwd(const float* g, const float* w, const float* 
     SeqGeom sg = make_seq_geom(B, T, F, axis);
     if (sg.n_seq == 0 || sg.L == 0) return 0;
     const long total = (long)sg.n_seq * cdiv(sg.L, CK);
-    glu_dwconv_fwd_kernel<<<resident_grid(total, 3), 256, 0, (cudaStream_t)stream>>>(g, sg, w, bias, out, bn_sums);
+    glu_dwconv_fwd_kernel<false><<<resident_grid(total, 3), 256, 0, (cudaStream_t)stream>>>(g, sg, w, bias, out, bn_sums, nullptr, B, axis);
+    return cmgan_check_launch("glu_dwconv_fwd_kernel");
+}
+
+// ragged batch (inference, no BatchNorm sums): utterance b has frames[b] valid frames; rows of frames t >= T_b are neither read nor written.
+// The grid is sized for the full (B, T) grid; the blocks split only the valid tiles between them.
+CMGAN_API int cmgan_glu_dwconv_fwd_ragged(const float* g, const float* w, const float* bias, int B, int T, int F, int axis, const int* frames,
+                                          float* out, void* stream) {
+    CMGAN_REQUIRE(g && w && bias && out && frames && (((uintptr_t)g) & 15) == 0, "cmgan_glu_dwconv_fwd_ragged: bad pointer");
+    CMGAN_REQUIRE(axis == 0 || axis == 1, "cmgan_glu_dwconv_fwd_ragged: bad axis");
+    SeqGeom sg = make_seq_geom(B, T, F, axis);
+    if (sg.n_seq == 0 || sg.L == 0) return 0;
+    const long total = (long)sg.n_seq * cdiv(sg.L, CK);
+    glu_dwconv_fwd_kernel<true><<<resident_grid(total, 3), 256, 0, (cudaStream_t)stream>>>(g, sg, w, bias, out, nullptr, frames, B, axis);
     return cmgan_check_launch("glu_dwconv_fwd_kernel");
 }
 

@@ -11,8 +11,11 @@ namespace {
 constexpr int NFFT = 400, HOP = 100, NF = 201;
 
 // ------------------------------------------------------------------ RMS scale: c[b] = sqrt(L / sum x^2)
-__global__ void rms_scale_kernel(const float* __restrict__ x, long ldx, int L, float* __restrict__ c) {
+// RAGGED: row b has its own length lens[b] (clamped to [0, L])
+template <bool RAGGED>
+__global__ void rms_scale_kernel(const float* __restrict__ x, long ldx, int L, float* __restrict__ c, const int* __restrict__ lens) {
     __shared__ double sm[32];
+    if (RAGGED) L = clamp_len(__ldg(lens + blockIdx.x), L);
     const float* p = x + (long)blockIdx.x * ldx;
     double s = 0.0;
     for (int i = threadIdx.x; i < L; i += blockDim.x) { float v = __ldg(p + i); s += (double)v * v; }
@@ -36,6 +39,29 @@ __global__ void pad_reflect_kernel(const float* __restrict__ x, long ldx, int L,
         int j = i - NFFT / 2;
         if (j < 0) j = -j;
         if (j >= L) j = 2 * (L - 1) - j;
+        v = __ldg(x + (long)b * ldx + j) * (c ? c[b] : 1.f);
+    }
+    xp[(long)b * Lp + i] = v;
+}
+
+// ragged front end of evaluation.py:21-29 + the STFT's centre padding: utterance b (L_b = lens[b] samples, clamped to [0, L]) is wrap-padded
+// with its own head to Lw = ceil(L_b / 100) * 100, reflect-padded by 200 on both sides and scaled by c[b]; zero from Lw + 400 up to Lp.
+// Needs L_b >= Lw - L_b and Lw > 200 (checked on the host); the value of every element is the one cmgan_pad_reflect gives the padded
+// utterance alone.
+__global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, const float* __restrict__ c,
+                                        float* __restrict__ xp, int Lp) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (i >= Lp) return;
+    const int Lb = clamp_len(__ldg(lens + b), L);
+    const int Lw = (Lb + HOP - 1) / HOP * HOP;
+    float v = 0.f;
+    if (Lb > 0 && i < Lw + NFFT) {
+        int j = i - NFFT / 2;
+        if (j < 0) j = -j;
+        if (j >= Lw) j = 2 * (Lw - 1) - j;
+        if (j >= Lb) j -= Lb;                         // wrap padding: sample Lb + k is sample k
+        j = clamp_len(j, Lb - 1);                     // only reachable for lengths the host rejects
         v = __ldg(x + (long)b * ldx + j) * (c ? c[b] : 1.f);
     }
     xp[(long)b * Lp + i] = v;
@@ -144,6 +170,33 @@ __global__ void ola_kernel(const float* __restrict__ frames, int T, const float*
     }
     s *= inv_env[n];
     if (c_div) s /= c_div[b];
+    y[(long)b * ldy + n] = s;
+}
+
+// overlap-add of a ragged batch: utterance b sums only its frames t < T_b = tlen[b] (clamped to [0, T]) into y[b, n], n < 100 (T_b - 1),
+// with its own inverse envelope: 1 / envelope(T_b) equals inv_env (the table of the full T-frame grid) except over the last 100 samples,
+// where frame T_b is missing; there it is inv_tail[n - 100 (T_b - 2)], the same for every T_b >= 4 (signal._inv_envelope_tail).
+// Samples n >= 100 (T_b - 1) are written as zero.
+__global__ void ola_ragged_kernel(const float* __restrict__ frames, int T, const int* __restrict__ tlen, const float* __restrict__ inv_env,
+                                  const float* __restrict__ inv_tail, const float* __restrict__ c_div, float* __restrict__ y, long ldy) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (n >= HOP * (T - 1)) return;
+    const int Tb = clamp_len(__ldg(tlen + b), T);
+    const int Lout = HOP * (Tb - 1);
+    float s = 0.f;
+    if (n < Lout) {
+        const int p = n + NFFT / 2;
+        int t_hi = p / HOP; if (t_hi > Tb - 1) t_hi = Tb - 1;
+        int t_lo = (p - NFFT + HOP) / HOP; if (p - NFFT + 1 <= 0) t_lo = 0;
+        for (int t = t_lo; t <= t_hi; ++t) {
+            const int k = p - t * HOP;
+            if (k >= 0 && k < NFFT) s += __ldg(frames + ((long)b * T + t) * NFFT + k);
+        }
+        const int tail0 = Lout - HOP;
+        s *= n >= tail0 ? inv_tail[n - tail0] : inv_env[n];
+        if (c_div) s /= c_div[b];
+    }
     y[(long)b * ldy + n] = s;
 }
 
@@ -360,8 +413,28 @@ __global__ void recombine_bwd_kernel(const float* __restrict__ m1, MaskTail mt, 
 CMGAN_API int cmgan_rms_scale(const float* x, long long ldx, int B, int L, float* c, void* stream) {
     CMGAN_REQUIRE(x && c && L > 0, "cmgan_rms_scale: bad arguments");
     if (B == 0) return 0;
-    rms_scale_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c);
+    rms_scale_kernel<false><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, nullptr);
     return cmgan_check_launch("rms_scale_kernel");
+}
+
+// c[b] = sqrt(L_b / sum_{i < L_b} x[b, i]^2), L_b = lengths[b] clamped to [0, L]
+CMGAN_API int cmgan_rms_scale_ragged(const float* x, long long ldx, int B, int L, const int* lengths, float* c, void* stream) {
+    CMGAN_REQUIRE(x && c && lengths && L > 0, "cmgan_rms_scale_ragged: bad arguments");
+    if (B == 0) return 0;
+    rms_scale_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, lengths);
+    return cmgan_check_launch("rms_scale_kernel");
+}
+
+// xp (B, Lp): utterance b wrap-padded to a multiple of 100, reflect-padded by 200 each side, scaled by c[b] (may be null), zero beyond;
+// Lp >= ceil(L / 100) * 100 + 400 covers every utterance
+CMGAN_API int cmgan_pad_wrap_reflect_ragged(const float* x, long long ldx, int B, int L, const int* lengths, const float* c, float* xp, int Lp,
+                                            void* stream) {
+    CMGAN_REQUIRE(x && xp && lengths && L > 0 && Lp >= (L + HOP - 1) / HOP * HOP + NFFT,
+                  "cmgan_pad_wrap_reflect_ragged: need Lp >= ceil(L / 100) * 100 + 400 (L=%d Lp=%d)", L, Lp);
+    if (B == 0) return 0;
+    dim3 grid(cdiv(Lp, 256), B);
+    pad_wrap_reflect_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, c, xp, Lp);
+    return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 
 // xp (B, Lp): reflect-padded (200 each side) and scaled by c[b] (c may be null); Lp >= L + 400, zero filled beyond
@@ -404,6 +477,15 @@ CMGAN_API int cmgan_ola(const float* frames, int B, int T, const float* inv_env,
     dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
     ola_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, inv_env, c_div, y, ldy);
     return cmgan_check_launch("ola_kernel");
+}
+
+CMGAN_API int cmgan_ola_ragged(const float* frames, int B, int T, const int* tlen, const float* inv_env, const float* inv_tail, const float* c_div,
+                               float* y, long long ldy, void* stream) {
+    CMGAN_REQUIRE(frames && tlen && inv_env && inv_tail && y && T >= 2, "cmgan_ola_ragged: bad arguments");
+    if (B == 0) return 0;
+    dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
+    ola_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, tlen, inv_env, inv_tail, c_div, y, ldy);
+    return cmgan_check_launch("ola_ragged_kernel");
 }
 
 CMGAN_API int cmgan_ola_bwd(const float* dy, long long lddy, int B, int T, const float* inv_env, float* dframes, void* stream) {

@@ -137,12 +137,23 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ d
 // ---------------------------------------------------------------- group statistics (InstanceNorm2d / BatchNorm1d)
 // sums[(grp*C + c)*2 + {0,1}] += sum x, sum x^2 over the rows of group grp.  Block = one chunk of rows of
 // one group; thread = (row-subgroup, channel).
+// RAGGED (InstanceNorm of a ragged batch): row = t * rows_per_t + f within a group, so the valid rows of group grp are the prefix
+// [0, T_grp * rows_per_t); chunks stay aligned at row 0, so every block partial equals the one a call over that utterance alone forms.
+template <bool RAGGED>
+__device__ __forceinline__ long stats_rows(long rows_per_group, long rows_per_t, const int* __restrict__ tlen, int grp) {
+    if (!RAGGED) return rows_per_group;
+    return (long)clamp_len(__ldg(tlen + grp), (int)(rows_per_group / rows_per_t)) * rows_per_t;
+}
+
+template <bool RAGGED>
 __global__ void norm_stats_kernel(const float* __restrict__ x, long ldx, long rows_per_group, int C, int chunk,
-                                  double* __restrict__ sums) {
+                                  double* __restrict__ sums, const int* __restrict__ tlen, long rows_per_t) {
     extern __shared__ double sm[];
     int grp = blockIdx.y;
     long r_beg = (long)blockIdx.x * chunk;
-    long r_end = r_beg + chunk < rows_per_group ? r_beg + chunk : rows_per_group;
+    const long n_rows = stats_rows<RAGGED>(rows_per_group, rows_per_t, tlen, grp);
+    if (RAGGED && r_beg >= n_rows) return;
+    long r_end = r_beg + chunk < n_rows ? r_beg + chunk : n_rows;
     int c = threadIdx.x % C, rg = threadIdx.x / C, nrg = blockDim.x / C;
     float s = 0.f, q = 0.f;
     const float* base = x + ((long)grp * rows_per_group) * ldx + c;
@@ -159,11 +170,15 @@ __global__ void norm_stats_kernel(const float* __restrict__ x, long ldx, long ro
 }
 
 // same, 128-bit loads: thread = (row-subgroup, 4 channels); C, ldx multiples of 4, x 16-byte aligned
-__global__ void norm_stats4_kernel(const float* __restrict__ x, long ldx, long rows_per_group, int C, int chunk, double* __restrict__ sums) {
+template <bool RAGGED>
+__global__ void norm_stats4_kernel(const float* __restrict__ x, long ldx, long rows_per_group, int C, int chunk, double* __restrict__ sums,
+                                   const int* __restrict__ tlen, long rows_per_t) {
     __shared__ float sm[256][8];
     const int grp = blockIdx.y, cv = C / 4;
     const long r_beg = (long)blockIdx.x * chunk;
-    const long r_end = r_beg + chunk < rows_per_group ? r_beg + chunk : rows_per_group;
+    const long n_rows = stats_rows<RAGGED>(rows_per_group, rows_per_t, tlen, grp);
+    if (RAGGED && r_beg >= n_rows) return;
+    const long r_end = r_beg + chunk < n_rows ? r_beg + chunk : n_rows;
     const int c4 = threadIdx.x % cv, rg = threadIdx.x / cv, nrg = blockDim.x / cv;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
     const float* base = x + ((long)grp * rows_per_group) * ldx + c4 * 4;
@@ -191,14 +206,17 @@ __global__ void norm_stats4_kernel(const float* __restrict__ x, long ldx, long r
 // mode 1: eval-mode BatchNorm: running statistics
 // outputs per (grp, c): scale = gamma*rstd, shift = beta - mean*scale, mean, rstd (table stride = tstride)
 // when running_mean != null and mode 0: running <- (1-mom)*running + mom*(mean, unbiased var) (BatchNorm1d train)
+// RAGGED (mode 0): group grp counts n = T_grp * rows_per_t rows (n is rows_per_t, T_max the frame count of the grid)
+template <bool RAGGED>
 __global__ void norm_finalize_kernel(const double* __restrict__ sums, long n, int G, int C, int mode,
                                      const float* __restrict__ gamma, const float* __restrict__ beta,
                                      float* __restrict__ running_mean, float* __restrict__ running_var, float momentum,
                                      float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ mean_out,
-                                     float* __restrict__ rstd_out, long tstride) {
+                                     float* __restrict__ rstd_out, long tstride, const int* __restrict__ tlen, int T_max) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= G * C) return;
     int grp = i / C, c = i % C;
+    if (RAGGED) n *= clamp_len(__ldg(tlen + grp), T_max);
     float mean, var;
     if (mode == 1) { mean = running_mean[c]; var = running_var[c]; }
     else {
@@ -510,13 +528,35 @@ CMGAN_API int cmgan_norm_stats(const float* x, long long ldx, int G, long long r
         const int nrg4 = 256 / (C / 4);
         const int chunk4 = nrg4 * 16;                 // 16 x 128-bit loads per thread; ~1000 blocks on the hot shapes
         dim3 grid4(cdiv(rows_per_group, chunk4), G);
-        norm_stats4_kernel<<<grid4, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk4, sums);
+        norm_stats4_kernel<false><<<grid4, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk4, sums, nullptr, 1);
         return cmgan_check_launch("norm_stats4_kernel");
     }
     int nrg = 256 / C;
     int chunk = nrg * 64;
     dim3 grid(cdiv(rows_per_group, chunk), G);
-    norm_stats_kernel<<<grid, norm_threads(C), 256 * 2 * sizeof(double), (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk, sums);
+    norm_stats_kernel<false><<<grid, norm_threads(C), 256 * 2 * sizeof(double), (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk, sums,
+                                                                                                       nullptr, 1);
+    return cmgan_check_launch("norm_stats_kernel");
+}
+
+// ragged batch: group g (utterance) sums only its first frames[g] * rows_per_frame rows (row = t * rows_per_frame + f within a group;
+// rows_per_group = T * rows_per_frame).  Same chunking as cmgan_norm_stats, so the block partials of a group equal those of a call over
+// that utterance alone.  sums must be zeroed by the caller.
+CMGAN_API int cmgan_norm_stats_ragged(const float* x, long long ldx, int G, long long rows_per_group, int C, long long rows_per_frame,
+                                      const int* frames, double* sums, void* stream) {
+    CMGAN_REQUIRE(x && sums && frames && C >= 1 && C <= 256 && 256 % C == 0, "cmgan_norm_stats_ragged: C=%d unsupported", C);
+    CMGAN_REQUIRE(rows_per_frame > 0 && rows_per_group % rows_per_frame == 0, "cmgan_norm_stats_ragged: rows_per_group must be a multiple of rows_per_frame");
+    if (G == 0 || rows_per_group == 0) return 0;
+    if (C % 4 == 0 && ldx % 4 == 0 && (((uintptr_t)x) & 15) == 0) {
+        const int chunk4 = 256 / (C / 4) * 16;
+        dim3 grid4(cdiv(rows_per_group, chunk4), G);
+        norm_stats4_kernel<true><<<grid4, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk4, sums, frames, rows_per_frame);
+        return cmgan_check_launch("norm_stats4_kernel");
+    }
+    const int chunk = 256 / C * 64;
+    dim3 grid(cdiv(rows_per_group, chunk), G);
+    norm_stats_kernel<true><<<grid, norm_threads(C), 256 * 2 * sizeof(double), (cudaStream_t)stream>>>(x, ldx, rows_per_group, C, chunk, sums,
+                                                                                                      frames, rows_per_frame);
     return cmgan_check_launch("norm_stats_kernel");
 }
 
@@ -525,9 +565,21 @@ CMGAN_API int cmgan_norm_finalize(const double* sums, long long n, int G, int C,
                                   float* mean_out, float* rstd_out, long long tstride, void* stream) {
     CMGAN_REQUIRE(gamma && beta && scale && shift, "cmgan_norm_finalize: null pointer");
     CMGAN_REQUIRE(mode == 1 ? (running_mean && running_var) : (sums != nullptr), "cmgan_norm_finalize: missing statistics");
-    norm_finalize_kernel<<<cdiv((long)G * C, 128), 128, 0, (cudaStream_t)stream>>>(sums, n, G, C, mode, gamma, beta, running_mean,
-                                                                                 running_var, momentum, scale, shift, mean_out,
-                                                                                 rstd_out, tstride);
+    norm_finalize_kernel<false><<<cdiv((long)G * C, 128), 128, 0, (cudaStream_t)stream>>>(sums, n, G, C, mode, gamma, beta, running_mean,
+                                                                                        running_var, momentum, scale, shift, mean_out,
+                                                                                        rstd_out, tstride, nullptr, 0);
+    return cmgan_check_launch("norm_finalize_kernel");
+}
+
+// InstanceNorm tables of a ragged batch (sums from cmgan_norm_stats_ragged): group g divides by its own count frames[g] * rows_per_frame
+// (frames clamped to [0, T])
+CMGAN_API int cmgan_norm_finalize_ragged(const double* sums, long long rows_per_frame, int T, const int* frames, int G, int C, const float* gamma,
+                                         const float* beta, float* scale, float* shift, float* mean_out, float* rstd_out, long long tstride,
+                                         void* stream) {
+    CMGAN_REQUIRE(sums && frames && gamma && beta && scale && shift, "cmgan_norm_finalize_ragged: null pointer");
+    norm_finalize_kernel<true><<<cdiv((long)G * C, 128), 128, 0, (cudaStream_t)stream>>>(sums, rows_per_frame, G, C, 0, gamma, beta, nullptr,
+                                                                                       nullptr, 0.f, scale, shift, mean_out, rstd_out, tstride,
+                                                                                       frames, T);
     return cmgan_check_launch("norm_finalize_kernel");
 }
 

@@ -105,6 +105,7 @@ struct Run {
     bool dry;
     int precision;
     cudaStream_t st;
+    const int* frames = nullptr;      // ragged batch: valid frames per utterance (device); null = every utterance fills the grid
     int rc = 0;
 
     const float* w(const std::string& key) const {
@@ -167,20 +168,27 @@ struct Gemm {
     }
 };
 
-void inst_norm_site(Run& r, const float* x, long long ldx, int G, long long rows, int Cn, const float* gamma, const float* beta, const Tabs& t,
-                    double*& sums) {
+// rows_per_t: rows of one frame within a group (row = t * rows_per_t + f); a ragged batch normalises over the valid frames only
+void inst_norm_site(Run& r, const float* x, long long ldx, int G, long long rows, long long rows_per_t, int Cn, const float* gamma, const float* beta,
+                    const Tabs& t, double*& sums) {
     double* s = sums;
     sums += (size_t)G * Cn * 2;
     if (!r.live()) return;
+    if (r.frames) {
+        r.ok(cmgan_norm_stats_ragged(x, ldx, G, rows, Cn, rows_per_t, r.frames, s, r.st));
+        r.ok(cmgan_norm_finalize_ragged(s, rows_per_t, (int)(rows / rows_per_t), r.frames, G, Cn, gamma, beta, t.scale, t.shift, t.mean, t.rstd,
+                                        t.width, r.st));
+        return;
+    }
     r.ok(cmgan_norm_stats(x, ldx, G, rows, Cn, s, r.st));
     r.ok(cmgan_norm_finalize(s, rows, G, Cn, 0, gamma, beta, nullptr, nullptr, 0.f, t.scale, t.shift, t.mean, t.rstd, t.width, r.st));
 }
 
 // InstanceNorm2d(affine) + PReLU of a raw (M, 64) tensor, written into dst (generator.py:35-37)
-void norm_prelu_to(Run& r, const float* raw, int G, long long rows, const float* gamma, const float* beta, const float* slope, float* dst,
-                   long long ldd, double*& sums) {
+void norm_prelu_to(Run& r, const float* raw, int G, long long rows, long long rows_per_t, const float* gamma, const float* beta, const float* slope,
+                   float* dst, long long ldd, double*& sums) {
     Tabs t = make_tabs(r, G, C);
-    inst_norm_site(r, raw, C, G, rows, C, gamma, beta, t, sums);
+    inst_norm_site(r, raw, C, G, rows, rows_per_t, C, gamma, beta, t, sums);
     if (r.live()) r.ok(cmgan_norm_apply(raw, C, G, rows, C, 1 | (r.precision == 1 ? 16 : 0), t.scale, t.shift, C, slope, dst, ldd, r.st));
 }
 
@@ -194,7 +202,7 @@ void dense_block(Run& r, float* cat, const std::string& p, int B, int T, int Fw,
         const int dy[6] = {-dil, -dil, -dil, 0, 0, 0}, dx[6] = {-1, 0, 1, -1, 0, 1};         // tap = kh * 3 + kw, causal in time (generator.py:12-21)
         Gemm(cat ? cat + c0 : nullptr, CAT, r.w(p + "conv" + s + ".weight"), 1, 6, (long long)Cin * 6, r.w(p + "conv" + s + ".bias"), raw, C, M, C, Cin)
             .taps(6, dy, dx).conv(T, Fw, T, Fw).run(r);
-        norm_prelu_to(r, raw, B, rows, r.w(p + "norm" + s + ".weight"), r.w(p + "norm" + s + ".bias"), r.w(p + "prelu" + s + ".weight"),
+        norm_prelu_to(r, raw, B, rows, Fw, r.w(p + "norm" + s + ".weight"), r.w(p + "norm" + s + ".bias"), r.w(p + "prelu" + s + ".weight"),
                       cat ? cat + co : nullptr, CAT, sums);
     }
 }
@@ -243,7 +251,11 @@ void conformer(Run& r, const float* x, float* y, const std::string& p, int B, in
     float* lse = r.alloc((size_t)M * 4);
     if (r.live()) {
         const float* E = r.w(p + "attn.fn.rel_pos_emb.weight");
-        r.ok(r.precision == 1 ? cmgan_attention_fwd_tf32(qkv, E, B, T, F2, axis, ctx, lse, r.st) : cmgan_attention_fwd(qkv, E, B, T, F2, axis, ctx, lse, r.st));
+        if (r.frames)
+            r.ok(r.precision == 1 ? cmgan_attention_fwd_tf32_ragged(qkv, E, B, T, F2, axis, r.frames, ctx, lse, r.st)
+                                  : cmgan_attention_fwd_ragged(qkv, E, B, T, F2, axis, r.frames, ctx, lse, r.st));
+        else
+            r.ok(r.precision == 1 ? cmgan_attention_fwd_tf32(qkv, E, B, T, F2, axis, ctx, lse, r.st) : cmgan_attention_fwd(qkv, E, B, T, F2, axis, ctx, lse, r.st));
     }
     float* x2 = r.alloc((size_t)M * C);
     Gemm(ctx, C, r.w(p + "attn.fn.to_out.weight"), 0, 1, C, r.w(p + "attn.fn.to_out.bias"), x2, C, M, C, C).residual(x1, C).run(r);
@@ -257,7 +269,10 @@ void conformer(Run& r, const float* x, float* y, const std::string& p, int B, in
     Tabs bn = make_tabs(r, 1, 2 * C);
     float* dsw = r.alloc((size_t)M * 2 * C);
     if (r.live()) {
-        r.ok(cmgan_glu_dwconv_fwd(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, d, nullptr, r.st));
+        if (r.frames)
+            r.ok(cmgan_glu_dwconv_fwd_ragged(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, r.frames, d, r.st));
+        else
+            r.ok(cmgan_glu_dwconv_fwd(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, d, nullptr, r.st));
         // eval: BatchNorm1d folds to scale / shift from the running statistics (mode 1; they are only read)
         r.ok(cmgan_norm_finalize(nullptr, M, 1, 2 * C, 1, r.w(p + "conv.net.5.weight"), r.w(p + "conv.net.5.bias"),
                                  const_cast<float*>(r.w(p + "conv.net.5.running_mean")), const_cast<float*>(r.w(p + "conv.net.5.running_var")), 0.1f,
@@ -292,14 +307,14 @@ void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt
         float* catE = r.alloc((size_t)M * CAT);
         float* raw0 = r.alloc((size_t)M * C);
         if (r.live()) r.ok(cmgan_head_conv(x, sxb, sxc, sxt, sxf, B, T, F, r.w(pe + "conv_1.0.weight"), r.w(pe + "conv_1.0.bias"), raw0, C, r.st));
-        norm_prelu_to(r, raw0, B, (long long)T * F, r.w(pe + "conv_1.1.weight"), r.w(pe + "conv_1.1.bias"), r.w(pe + "conv_1.2.weight"),
+        norm_prelu_to(r, raw0, B, (long long)T * F, F, r.w(pe + "conv_1.1.weight"), r.w(pe + "conv_1.1.bias"), r.w(pe + "conv_1.2.weight"),
                       catE ? catE + 4 * C : nullptr, CAT, sums);
         dense_block(r, catE, pe + "dilated_dense.", B, T, F, sums);
         float* e2 = r.alloc((size_t)M2 * C);
         const int dy[3] = {0, 0, 0}, dx[3] = {-1, 0, 1};
         Gemm(catE, CAT, r.w(pe + "conv_2.0.weight"), 1, 3, 3 * C, r.w(pe + "conv_2.0.bias"), e2, C, M2, C, C).taps(3, dy, dx).conv(T, F2, T, F, 2).run(r);
         Tabs t2 = make_tabs(r, B, C);
-        inst_norm_site(r, e2, C, B, (long long)T * F2, C, r.w(pe + "conv_2.1.weight"), r.w(pe + "conv_2.1.bias"), t2, sums);
+        inst_norm_site(r, e2, C, B, (long long)T * F2, F2, C, r.w(pe + "conv_2.1.weight"), r.w(pe + "conv_2.1.bias"), t2, sums);
         if (r.live()) r.ok(cmgan_norm_apply(e2, C, B, (long long)T * F2, C, 1, t2.scale, t2.shift, C, r.w(pe + "conv_2.2.weight"), hA, C, r.st));
         r.top = mark;
     }
@@ -330,8 +345,8 @@ void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt
     Tabs tabM = make_tabs(r, B, 1), tabC = make_tabs(r, B, C);
     float* cplx = r.alloc((size_t)M * 2);
     if (r.live()) r.ok(cmgan_rowdot_fwd(sp[0], B, T, F, 1, nullptr, nullptr, nullptr, r.w(pm + "conv_1.weight"), r.w(pm + "conv_1.bias"), m1, r.st));
-    inst_norm_site(r, m1, 1, B, (long long)T * F, 1, r.w(pm + "norm.weight"), r.w(pm + "norm.bias"), tabM, sums);
-    inst_norm_site(r, sp[1], C, B, (long long)T * 2 * F2, C, r.w(pc + "norm.weight"), r.w(pc + "norm.bias"), tabC, sums);
+    inst_norm_site(r, m1, 1, B, (long long)T * F, F, 1, r.w(pm + "norm.weight"), r.w(pm + "norm.bias"), tabM, sums);
+    inst_norm_site(r, sp[1], C, B, (long long)T * 2 * F2, 2 * F2, C, r.w(pc + "norm.weight"), r.w(pc + "norm.bias"), tabC, sums);
     if (r.live()) {
         r.ok(cmgan_rowdot_fwd(sp[1], B, T, F, 2, tabC.scale, tabC.shift, r.w(pc + "prelu.weight"), r.w(pc + "conv.weight"), r.w(pc + "conv.bias"), cplx, r.st));
         r.ok(cmgan_recombine(m1, tabM.scale, tabM.shift, r.w(pm + "prelu.weight"), r.w(pm + "final_conv.weight"), r.w(pm + "final_conv.bias"),
@@ -362,8 +377,8 @@ CMGAN_API long long cmgan_tscnet_workspace_bytes(int B, int T, int F, int precis
     return (long long)r.peak + 256;
 }
 
-CMGAN_API int cmgan_tscnet_fwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
-                               float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream) {
+static int tscnet_fwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
+                      const int* frames, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream) {
     CMGAN_REQUIRE(params && x && final_real && final_imag && workspace, "cmgan_tscnet_fwd: null pointer");
     CMGAN_REQUIRE(B > 0 && T > 0 && F == NFEAT, "cmgan_tscnet_fwd: expected x of shape (B, 2, T, %d), got B=%d T=%d F=%d", NFEAT, B, T, F);
     CMGAN_REQUIRE(precision == 0 || precision == 1, "cmgan_tscnet_fwd: precision must be 0 (fp32) or 1 (tf32)");
@@ -372,6 +387,24 @@ CMGAN_API int cmgan_tscnet_fwd(const float* params, const float* x, long long sx
     Run r;
     r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
     r.st = (cudaStream_t)stream;
+    r.frames = frames;
     forward(r, x, sxb, sxc, sxt, sxf, B, T, F, final_real, final_imag);
     return r.rc;
+}
+
+CMGAN_API int cmgan_tscnet_fwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
+                               float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream) {
+    return tscnet_fwd(params, x, sxb, sxc, sxt, sxf, B, T, F, nullptr, final_real, final_imag, workspace, workspace_bytes, precision, stream);
+}
+
+// ragged batch: utterance b occupies frames t < frames[b]; the InstanceNorms, the attention and the depthwise convolutions see only those
+// frames, everything else works per row or causally in time (the dense blocks' dilated convolutions pad only the past)
+CMGAN_API int cmgan_tscnet_fwd_ragged(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T,
+                                      int F, const int* frames, float* final_real, float* final_imag, void* workspace, long long workspace_bytes,
+                                      int precision, void* stream) {
+    CMGAN_REQUIRE(frames, "cmgan_tscnet_fwd_ragged: frames is null");
+    CMGAN_REQUIRE(B > 0 && T > 0 && (long long)B * T * F * CAT < (1ll << 31),
+                  "cmgan_tscnet_fwd_ragged: B * T * F * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split the batch",
+                  CAT, (long long)B * T * F * CAT);
+    return tscnet_fwd(params, x, sxb, sxc, sxt, sxf, B, T, F, frames, final_real, final_imag, workspace, workspace_bytes, precision, stream);
 }

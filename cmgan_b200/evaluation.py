@@ -6,9 +6,12 @@ the signal's own head, fold files longer than ``cut_len`` into a batch, STFT -> 
 is absent here; 16-bit PCM, 32-bit float and 32-bit PCM files are read to float32 in [-1, 1) exactly as torchaudio does, float32 is
 written like soundfile's default for float input would be on a FLOAT-subtype file -- pass ``subtype='PCM_16'`` for 16-bit output).
 
-``enhance_files`` is the throughput front-end for the config-5 sweep: files are bucketed by padded length (InstanceNorm statistics span
-the whole (T, F) plane, so only clips of identical length can share a batch without changing any output) and every bucket goes through
-the network as one batch.
+``enhance_files`` is the throughput front end: files of different lengths share ragged batches (``plan_batches``: sorted by length, at
+most ``max_batch`` files and fewer than 2^31 elements in the widest buffer per batch) and go through ``signal.enhance_ragged``, where each
+utterance occupies the first T_b frames of a (B, T_max) grid and the operators that mix frames -- InstanceNorm statistics, time-axis
+attention, the time-axis depthwise convolution, the inverse STFT's overlap-add -- see only those frames.  Every output equals the per-file
+result (up to the order of the double-precision atomic sums of the InstanceNorm statistics).  Files longer than ``cut_len`` take the
+reference's folding path one at a time.
 """
 from __future__ import annotations
 
@@ -22,6 +25,7 @@ import torch
 from . import signal
 
 SR = 16000
+MAX_ELEMENTS = 2 ** 31          # the widest activation buffer (B * T * 201 * 320 floats) is indexed with 32-bit element counts
 
 
 def read_wav(path: str) -> Tuple[torch.Tensor, int]:
@@ -75,39 +79,73 @@ def enhance_one_track(model, audio_path: str, saved_dir: Optional[str], cut_len:
     return est_audio, length
 
 
+def plan_batches(lengths: Sequence[int], cut_len: int = SR * 16, max_batch: int = 16) -> Tuple[List[List[int]], List[int]]:
+    """Pure host planning of ``enhance_files``: sample counts -> (ragged batches as lists of indices into ``lengths``, indices of the files
+    longer than ``cut_len`` after padding, which take the folding path alone).  Files are sorted by length (ties by index), so a batch
+    holds neighbours and little padding; a batch closes at ``max_batch`` files or before B * T_max * 201 * 320 reaches 2^31.  Raises
+    ValueError for a clip too short for the wrap padding (``signal.ragged_padded_length``)."""
+    if max_batch < 1:
+        raise ValueError("max_batch must be >= 1")
+    solo, fit = [], []
+    for i, L in enumerate(lengths):
+        padded = int(np.ceil(L / 100)) * 100
+        if padded > cut_len:
+            solo.append(i)
+        else:
+            signal.ragged_padded_length(int(L), cut_len)
+            fit.append(i)
+    fit.sort(key=lambda i: (lengths[i], i))
+    batches: List[List[int]] = []
+    cur: List[int] = []
+    for i in fit:
+        T = signal.ragged_padded_length(int(lengths[i]), cut_len) // signal.HOP + 1      # the widest clip so far: it sets T_max
+        if cur and (len(cur) >= max_batch or (len(cur) + 1) * T * signal.NF * 320 >= MAX_ELEMENTS):
+            batches.append(cur)
+            cur = []
+        cur.append(i)
+    if cur:
+        batches.append(cur)
+    return batches, solo
+
+
+def padding_waste(lengths: Sequence[int], batches: Sequence[Sequence[int]], cut_len: int = SR * 16) -> float:
+    """1 - sum_b T_b / sum_batches (B * T_max): the share of the frame grid that ragged batching spends on padding"""
+    used = grid = 0
+    for part in batches:
+        T = [signal.ragged_padded_length(int(lengths[i]), cut_len) // signal.HOP + 1 for i in part]
+        used += sum(T)
+        grid += len(T) * max(T)
+    return 1.0 - used / grid if grid else 0.0
+
+
 @torch.no_grad()
 def enhance_files(model, paths: Sequence[str], cut_len: int = SR * 16, max_batch: int = 16) -> Dict[str, np.ndarray]:
-    """Enhance many files with identical-length clips batched together (bit-for-bit the per-file results: nothing is padded or mixed).
-    Files longer than ``cut_len`` take the reference's folding path one at a time."""
+    """Enhance many files, packed into ragged batches of up to ``max_batch`` files of different lengths (``plan_batches``); every output
+    equals the per-file result.  Files longer than ``cut_len`` take the reference's folding path one at a time."""
     dev = next(model.parameters()).device
-    waves, buckets = {}, {}
+    waves = []
     for p in paths:
         x, sr = read_wav(p)
         assert sr == SR
-        waves[p] = x[:1]
-        L = x.size(-1)
-        key = L if int(np.ceil(L / 100)) * 100 <= cut_len else ("solo", p)
-        buckets.setdefault(key, []).append(p)
+        waves.append(x[0])
+    batches, solo = plan_batches([w.numel() for w in waves], cut_len, max_batch)
     out: Dict[str, np.ndarray] = {}
-    for key, group in buckets.items():
-        if isinstance(key, tuple):
-            out[group[0]] = signal.enhance(model, waves[group[0]].to(dev), cut_len=cut_len).cpu().numpy()
-            continue
-        for i in range(0, len(group), max_batch):
-            part = group[i:i + max_batch]
-            batch = torch.cat([waves[p] for p in part], dim=0).to(dev)
-            est = signal.enhance_batch(model, batch)
-            for p, e in zip(part, est):
-                out[p] = e.cpu().numpy()
+    for i in solo:
+        out[paths[i]] = signal.enhance(model, waves[i][None].to(dev), cut_len=cut_len).cpu().numpy()
+    for part in batches:
+        est = signal.enhance_ragged(model, [waves[i].to(dev) for i in part], cut_len=cut_len)
+        for i, e in zip(part, est):
+            out[paths[i]] = e.cpu().numpy()
     return out
 
 
 @torch.no_grad()
 def evaluation(model, noisy_dir: str, clean_dir: str, save_tracks: bool, saved_dir: str,
-               metrics: Optional[Callable[[np.ndarray, np.ndarray], Sequence[float]]] = None, cut_len: int = SR * 16):
+               metrics: Optional[Callable[[np.ndarray, np.ndarray], Sequence[float]]] = None, cut_len: int = SR * 16, max_batch: int = 1):
     """reference evaluation.py:60-97 with an already-loaded ``model``: enhance every file of ``noisy_dir`` in natural order, score it against
     the file of the same name in ``clean_dir`` with ``metrics(clean, enhanced) -> sequence`` (default: the PESQ-free pair SSNR, STOI from
-    cmgan_b200.metrics on the GPU) and return the per-metric averages."""
+    cmgan_b200.metrics on the GPU) and return the per-metric averages.  ``max_batch`` > 1 enhances through ``enhance_files`` (ragged
+    batches, same outputs) first and then scores in the same natural order; the default 1 is the reference's per-file loop."""
     model.eval()
     if save_tracks and not os.path.exists(saved_dir):
         os.mkdir(saved_dir)
@@ -118,9 +156,18 @@ def evaluation(model, noisy_dir: str, clean_dir: str, save_tracks: bool, saved_d
         def metrics(clean, est):
             return gpu_metrics.ssnr_stoi(torch.from_numpy(clean).to(dev), torch.from_numpy(est).to(dev))
     names = natural_sorted(os.listdir(noisy_dir))
+    batched = None
+    if max_batch > 1:
+        batched = enhance_files(model, [os.path.join(noisy_dir, n) for n in names], cut_len=cut_len, max_batch=max_batch)
     total = None
     for name in names:
-        est_audio, length = enhance_one_track(model, os.path.join(noisy_dir, name), saved_dir, cut_len, 400, 100, save_tracks)
+        if batched is None:
+            est_audio, length = enhance_one_track(model, os.path.join(noisy_dir, name), saved_dir, cut_len, 400, 100, save_tracks)
+        else:
+            est_audio = batched[os.path.join(noisy_dir, name)]
+            length = len(est_audio)
+            if save_tracks:
+                write_wav(os.path.join(saved_dir, name), est_audio, SR)
         clean, sr = read_wav(os.path.join(clean_dir, name))
         assert sr == SR
         m = np.asarray(metrics(clean[0].numpy()[:length], est_audio), dtype=np.float64)

@@ -217,11 +217,17 @@ class TSCNet(nn.Module):
         G = {k: torch.zeros_like(named[k]) for k in self._param_keys}
         return G, tuple(G[k] if named[k].requires_grad else None for k in self._param_keys)
 
-    def forward(self, x: torch.Tensor):
+    def forward(self, x: torch.Tensor, frames=None):
+        """``frames`` (optional, inference only): a (B,) int sequence or tensor -- a ragged batch in which utterance b occupies frames
+        t < frames[b] of x's (B, 2, T, F) grid, 1 <= frames[b] <= T.  Input frames past an utterance's end are never read (they may hold
+        anything); its output frames there are unspecified.  Each utterance's valid frames equal a forward of that utterance alone, up to the
+        order of the double-precision atomic sums of the InstanceNorm statistics."""
         if not x.is_cuda:
             raise RuntimeError("cmgan_b200.TSCNet runs on CUDA only (no CPU fallback)")
         if x.dtype != torch.float32:
             raise RuntimeError("cmgan_b200.TSCNet expects float32 input")
+        if frames is not None:
+            return self._forward_ragged(x, frames)
         if self.training:
             self._step += 1
             torch._foreach_add_([b for k, b in self.named_buffers() if k.endswith("num_batches_tracked")], 1)   # bookkeeping only
@@ -239,3 +245,29 @@ class TSCNet(nn.Module):
             finally:
                 ops.PACK_CACHE = None
         return _TSCNetFn.apply(x, self, self.training, self.seed * 7919 + self._step, *params)
+
+    def _forward_ragged(self, x: torch.Tensor, frames):
+        if self.training or torch.is_grad_enabled():
+            raise RuntimeError("TSCNet.forward(frames=...) is inference only: call model.eval() and run under torch.no_grad() "
+                               "(the backward kernels and train-mode BatchNorm have no ragged form)")
+        if x.dim() != 4 or x.shape[1] != 2:
+            raise RuntimeError(f"expected x of shape (B, 2, T, F), got {tuple(x.shape)}")
+        B, _, T, _ = x.shape
+        fr_host = torch.as_tensor(frames).detach().to("cpu", torch.int64).reshape(-1)
+        if fr_host.numel() != B:
+            raise ValueError(f"frames has {fr_host.numel()} entries for a batch of {B}")
+        if B and (int(fr_host.min()) < 1 or int(fr_host.max()) > T):
+            raise ValueError(f"frames must lie in [1, T = {T}], got {fr_host.tolist()}")
+        fdev = fr_host.to(torch.int32).to(x.device)
+        params = [p for _, p in self.named_parameters()]
+        sig = (params[0].data_ptr(), sum(p._version for p in params), self._weights_epoch)
+        if sig != self._pack_sig:
+            self._pack.clear()
+            self._pack_sig = sig
+        if ops.PACK_CACHE is not None:
+            return tscnet_fwd(x, self._tensor_dict(), False, 0, None, frames=fdev)
+        ops.PACK_CACHE = self._pack          # frozen weights: the re-tiled tensor-core copies are kept between calls, as in forward()
+        try:
+            return tscnet_fwd(x, self._tensor_dict(), False, 0, None, frames=fdev)
+        finally:
+            ops.PACK_CACHE = None

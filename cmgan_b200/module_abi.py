@@ -40,8 +40,10 @@ def workspace_bytes(B: int, T: int, F: int, precision: int) -> int:
     return n
 
 
-def tscnet_forward(flat: torch.Tensor, x: torch.Tensor, precision: int = 1, workspace: torch.Tensor = None):
-    """x (B, 2, T, F) on the GPU, any strides -> (final_real, final_imag), each (B, 1, T, F)"""
+def tscnet_forward(flat: torch.Tensor, x: torch.Tensor, precision: int = 1, workspace: torch.Tensor = None, frames=None):
+    """x (B, 2, T, F) on the GPU, any strides -> (final_real, final_imag), each (B, 1, T, F).
+    ``frames``: optional ragged batch (device int32 (B,) tensor, or anything torch.as_tensor takes): utterance b occupies frames t < frames[b]
+    (``cmgan_tscnet_fwd_ragged``; output frames past that are unspecified).  The workspace size is the same as for the uniform call."""
     assert x.is_cuda and flat.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 2
     B, _, T, F = x.shape
     if workspace is None:
@@ -49,6 +51,13 @@ def tscnet_forward(flat: torch.Tensor, x: torch.Tensor, precision: int = 1, work
     fr = torch.empty(B, 1, T, F, device=x.device)
     fi = torch.empty(B, 1, T, F, device=x.device)
     sb, sc, st, sf = x.stride()
-    lib().call("cmgan_tscnet_fwd", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, fr.data_ptr(), fi.data_ptr(), workspace.data_ptr(),
-               workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    stream = torch.cuda.current_stream().cuda_stream
+    if frames is None:
+        lib().call("cmgan_tscnet_fwd", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, fr.data_ptr(), fi.data_ptr(), workspace.data_ptr(),
+                   workspace.numel(), precision, stream)
+    else:
+        fdev = torch.as_tensor(frames, dtype=torch.int32, device=x.device).reshape(-1).contiguous()
+        assert fdev.numel() == B, f"frames has {fdev.numel()} entries for a batch of {B}"
+        lib().call("cmgan_tscnet_fwd_ragged", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, fdev.data_ptr(), fr.data_ptr(), fi.data_ptr(),
+                   workspace.data_ptr(), workspace.numel(), precision, stream)
     return fr, fi

@@ -8,7 +8,7 @@ inverse basis followed by overlap-add.  Both run in exact fp32 FFMA (0.1 GFLOP p
 from __future__ import annotations
 
 import math
-from typing import Dict, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 import torch
 
@@ -64,6 +64,15 @@ def _inv_envelope(T: int, dev) -> torch.Tensor:
     return _CACHE[key]
 
 
+def _inv_envelope_tail(dev) -> torch.Tensor:
+    """the last 100 samples of 1 / envelope(T), the same for every T >= 3: at n >= 100 (T - 2) frame T is missing, elsewhere envelope(T)
+    equals envelope(T') for any T' >= T (the ragged overlap-add combines this tail with the table of the longest utterance)"""
+    key = ("env_tail", dev)
+    if key not in _CACHE:
+        _CACHE[key] = _inv_envelope(8, dev)[600:700].contiguous()
+    return _CACHE[key]
+
+
 def rms_scale(wav: torch.Tensor) -> torch.Tensor:
     """c[b] = sqrt(L / sum x^2)  (ref: train.py:75, evaluation.py:21)"""
     assert wav.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
@@ -83,16 +92,25 @@ def stft_compress(wav: torch.Tensor, scale: torch.Tensor = None) -> torch.Tensor
     Lp = ((L + N_FFT + HOP - 1) // HOP) * HOP
     xp = torch.empty(B, Lp, device=dev)
     call("cmgan_pad_reflect", wav, wav.stride(0), B, L, scale, xp, Lp)
+    return _stft_padded(xp, B, T).permute(0, 1, 3, 2)
+
+
+def _stft_padded(xp: torch.Tensor, B: int, T: int) -> torch.Tensor:
+    """(B, Lp) centre-padded waveforms -> power-compressed spectrogram (B, 2, T, F), contiguous; frame t reads xp[:, 100 t : 100 t + 400]"""
+    dev = xp.device
+    Lp = xp.shape[1]
     S = torch.empty(B * T, 2 * NF, device=dev)
     gemm(A=xp, lda=HOP, W=_fwd_basis(dev), sb_k=2 * NF, sb_n=1, C=S, ldc=2 * NF, M=B * T, N=2 * NF, Cin=N_FFT, taps=[(0, 0)],
          conv=dict(OH=1, OW=T, IH=1, IW=Lp // HOP), precision=0)      # the DFTs stay exact fp32
     X = torch.empty(B, 2, T, NF, device=dev)
     call("cmgan_compress", S, B, T, X)
-    return X.permute(0, 1, 3, 2)
+    return X
 
 
-def uncompress_istft_fwd(fr: torch.Tensor, fi: torch.Tensor, c_div: torch.Tensor = None) -> torch.Tensor:
-    """un-compress (B,1,T,F) x 2 -> inverse DFT (GEMM) -> overlap-add -> (B, 100 (T-1)); no autograd"""
+def uncompress_istft_fwd(fr: torch.Tensor, fi: torch.Tensor, c_div: torch.Tensor = None, tlen: torch.Tensor = None) -> torch.Tensor:
+    """un-compress (B,1,T,F) x 2 -> inverse DFT (GEMM) -> overlap-add -> (B, 100 (T-1)); no autograd.
+    ``tlen`` (ragged batch, device int32 (B,)): utterance b has tlen[b] >= 3 valid frames and gets y[b, :100 (tlen[b] - 1)], overlap-added
+    from those frames alone with its own envelope (zeros after)."""
     dev = fr.device
     B, _, T, F = fr.shape
     assert F == NF and fi.stride() == fr.stride()
@@ -102,7 +120,10 @@ def uncompress_istft_fwd(fr: torch.Tensor, fi: torch.Tensor, c_div: torch.Tensor
     frames = torch.empty(B * T, N_FFT, device=dev)
     gemm(A=U, lda=2 * NF, W=_inv_basis(dev), sb_k=N_FFT, sb_n=1, C=frames, ldc=N_FFT, M=B * T, N=N_FFT, Cin=2 * NF, precision=0)
     y = torch.empty(B, HOP * (T - 1), device=dev)
-    call("cmgan_ola", frames, B, T, _inv_envelope(T, dev), c_div, y, y.stride(0))
+    if tlen is not None:
+        call("cmgan_ola_ragged", frames, B, T, tlen, _inv_envelope(T, dev), _inv_envelope_tail(dev), c_div, y, y.stride(0))
+    else:
+        call("cmgan_ola", frames, B, T, _inv_envelope(T, dev), c_div, y, y.stride(0))
     return y
 
 
@@ -182,3 +203,51 @@ def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16) -> torch.Tens
     fr, fi = model(spec)
     audio = uncompress_istft(fr, fi, cb)
     return audio.reshape(-1)[:length]
+
+
+def ragged_padded_length(length: int, cut_len: int = 16000 * 16) -> int:
+    """Length of a clip after the wrap padding to a multiple of 100 (evaluation.py:25-29), checked for a ragged batch: the padding is
+    taken from the clip's own head, so it may not be longer than the clip; the padded clip must exceed the 200-sample reflect padding of the
+    STFT and fit in ``cut_len`` (longer files take the folding path of ``enhance``).  Raises ValueError otherwise."""
+    padded = int(math.ceil(length / 100)) * 100
+    if padded - length > length or padded <= N_FFT // 2:
+        raise ValueError(f"a clip of {length} samples is too short: wrap padding to {padded} and the 200-sample reflect padding need "
+                         f"at least {max(padded - length, N_FFT // 2 + 1)} samples")
+    if padded > cut_len:
+        raise ValueError(f"a clip of {length} samples (padded {padded}) is longer than cut_len = {cut_len}")
+    return padded
+
+
+@torch.no_grad()
+def enhance_ragged(model, waves: Sequence[torch.Tensor], cut_len: int = 16000 * 16) -> List[torch.Tensor]:
+    """Enhance clips of different lengths in ONE batch: ``waves`` = 1-D float32 CUDA waveforms, each no longer than ``cut_len`` after the
+    wrap padding -> the list of enhanced waveforms, each what ``enhance`` returns for that clip alone.
+
+    The clips share a (B, T_max) frame grid; clip b occupies its first T_b = padded_b / 100 + 1 frames.  Every stage runs on the ragged
+    kernels: RMS scale and wrap + reflect padding per clip length, the framed DFT (per frame), the TSCNet forward with ``frames`` = T_b, the
+    inverse DFT (per frame) and an overlap-add that sums each clip's own frames with its own envelope, then de-normalises."""
+    if len(waves) == 0:
+        return []
+    dev = waves[0].device
+    for w in waves:
+        if not (w.is_cuda and w.dtype == torch.float32 and w.dim() == 1 and w.device == dev):
+            raise ValueError("enhance_ragged expects 1-D float32 CUDA waveforms on one device")
+    lens = [int(w.numel()) for w in waves]
+    tframes = [ragged_padded_length(L, cut_len) // HOP + 1 for L in lens]
+    B, Lmax, Tmax = len(waves), max(lens), max(tframes)
+    x = torch.zeros(B, Lmax, device=dev)
+    for b, w in enumerate(waves):
+        x[b, :lens[b]].copy_(w)
+    meta = torch.tensor([lens, tframes], dtype=torch.int32).to(dev)           # one host-to-device copy: sample and frame counts
+    ln, tb = meta[0], meta[1]
+    c = torch.empty(B, device=dev)
+    call("cmgan_rms_scale_ragged", x, x.stride(0), B, Lmax, ln, c)
+    Lp = (Tmax - 1) * HOP + N_FFT
+    xp = torch.empty(B, Lp, device=dev)
+    call("cmgan_pad_wrap_reflect_ragged", x, x.stride(0), B, Lmax, ln, c, xp, Lp)
+    spec = _stft_padded(xp, B, Tmax)
+    fr, fi = model(spec, frames=tframes)
+    if fi.stride() != fr.stride():
+        fr, fi = fr.contiguous(), fi.contiguous()
+    y = uncompress_istft_fwd(fr, fi, c, tb)
+    return [y[b, :lens[b]] for b in range(B)]

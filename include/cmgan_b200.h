@@ -45,6 +45,8 @@ int cmgan_norm_finalize(const double* sums, long long n, int G, int C, int mode,
 int cmgan_norm_bwd_reduce(const float* x, long long ldx, const float* dact, long long ldd, int G, long long rows_per_group, int C, int act, const float* scale, const float* shift, const float* mean, const float* rstd, long long tstride, const float* slope, double* S, float* dslope, void* stream);
 int cmgan_norm_bwd_apply(const float* x, long long ldx, const float* dact, long long ldd, int G, long long rows_per_group, int C, int act, int use_batch_stats, const float* scale, const float* shift, const float* mean, const float* rstd, long long tstride, const float* slope, const double* S, float* dx, long long lddx, float* dgamma, float* dbeta, void* stream);
 int cmgan_norm_apply(const float* x, long long ldx, int G, long long rows_per_group, int C, int act, const float* scale, const float* shift, long long tstride, const float* slope, float* y, long long ldy, void* stream);
+int cmgan_norm_stats_ragged(const float* x, long long ldx, int G, long long rows_per_group, int C, long long rows_per_frame, const int* frames, double* sums, void* stream);
+int cmgan_norm_finalize_ragged(const double* sums, long long rows_per_frame, int T, const int* frames, int G, int C, const float* gamma, const float* beta, float* scale, float* shift, float* mean_out, float* rstd_out, long long tstride, void* stream);
 int cmgan_fill(float* p, long long n, float v, void* stream);
 int cmgan_copy_rows(const float* src, long long lds, float* dst, long long ldd, long long M, int C, void* stream);
 int cmgan_copy_rows_operand(const float* src, long long lds, float* dst, long long ldd, long long M, int C, void* stream);
@@ -53,6 +55,8 @@ int cmgan_add_rows(const float* src, long long lds, float* dst, long long ldd, l
 /* ---- attention with Shaw relative positions (conformer.py:100-131); axis 0 = time sequences, 1 = frequency sequences */
 int cmgan_attention_fwd(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, void* stream);
 int cmgan_attention_fwd_tf32(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, void* stream);
+int cmgan_attention_fwd_ragged(const float* qkv, const float* E, int B, int T, int F, int axis, const int* frames, float* ctx, float* lse, void* stream);
+int cmgan_attention_fwd_tf32_ragged(const float* qkv, const float* E, int B, int T, int F, int axis, const int* frames, float* ctx, float* lse, void* stream);
 int cmgan_attention_fwd_tf32_nbuf(const float* qkv, const float* E, int B, int T, int F, int axis, float* ctx, float* lse, int nbuf, void* stream);
 int cmgan_attention_bwd(const float* qkv, const float* E, const float* ctx, const float* dctx, const float* lse, int B, int T, int F, int axis, float* delta, float* dqkv, float* dE, void* stream);
 int cmgan_attention_bwd_tf32_parts(const float* qkv, const float* E, const float* ctx, const float* dctx, const float* lse, int B, int T, int F, int axis, float* delta, float* dqkv, float* dE, int parts, void* stream);
@@ -62,17 +66,21 @@ int cmgan_attention_bwd_tf32(const float* qkv, const float* E, const float* ctx,
 
 /* ---- GLU + depthwise conv k=31 (conformer.py:30-48,164-168) */
 int cmgan_glu_dwconv_fwd(const float* g, const float* w, const float* bias, int B, int T, int F, int axis, float* out, double* bn_sums, void* stream);
+int cmgan_glu_dwconv_fwd_ragged(const float* g, const float* w, const float* bias, int B, int T, int F, int axis, const int* frames, float* out, void* stream);
 int cmgan_glu_dwconv_bwd(const float* g, const float* dz, const float* w, int B, int T, int F, int axis, float* dg, float* dw, float* dbias, void* stream);
 
 /* ---- signal front / back end (train.py:75-112, evaluation.py:21-51, utils.py:20-39) */
 int cmgan_rms_scale(const float* x, long long ldx, int B, int L, float* c, void* stream);
 int cmgan_pad_reflect(const float* x, long long ldx, int B, int L, const float* c, float* xp, int Lp, void* stream);
+int cmgan_rms_scale_ragged(const float* x, long long ldx, int B, int L, const int* lengths, float* c, void* stream);
+int cmgan_pad_wrap_reflect_ragged(const float* x, long long ldx, int B, int L, const int* lengths, const float* c, float* xp, int Lp, void* stream);
 int cmgan_compress(const float* S, int B, int T, float* X, void* stream);
 int cmgan_uncompress(const float* re, const float* im, long long sb, long long st, long long sf, int B, int T, float* U, void* stream);
 int cmgan_uncompress_bwd(const float* re, const float* im, long long sb, long long st, long long sf, int B, int T, const float* dU, float* dre, float* dim_, int accumulate, void* stream);
 int cmgan_power_law(const float* re, const float* im, long long i0, long long i1, long long i2, float* ore, float* oim, long long o0, long long o1, long long o2, int d0, int d1, int d2, float p, void* stream);
 int cmgan_power_law_bwd(const float* re, const float* im, long long i0, long long i1, long long i2, const float* gre, const float* gim, long long o0, long long o1, long long o2, float* dre, float* dim_, long long q0, long long q1, long long q2, int d0, int d1, int d2, float p, void* stream);
 int cmgan_ola(const float* frames, int B, int T, const float* inv_env, const float* c_div, float* y, long long ldy, void* stream);
+int cmgan_ola_ragged(const float* frames, int B, int T, const int* tlen, const float* inv_env, const float* inv_tail, const float* c_div, float* y, long long ldy, void* stream);
 int cmgan_ola_bwd(const float* dy, long long lddy, int B, int T, const float* inv_env, float* dframes, void* stream);
 
 /* ---- generator head and tails (generator.py:53,126,136-139,150,175-196) */
@@ -122,6 +130,13 @@ long long cmgan_tscnet_param_floats(void);
 int cmgan_tscnet_param_info(int index, const char** key, long long* offset, long long* numel);
 long long cmgan_tscnet_workspace_bytes(int B, int T, int F, int precision);
 int cmgan_tscnet_fwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
+/* Ragged batch: utterance b occupies frames t < frames[b] of the (B, 2, T, F) grid (frames: device int32[B], 1 <= T_b <= T; values are
+ * clamped to [0, T] on the device).  Input frames t >= T_b are never read and may hold anything, NaN included; output frames t >= T_b are
+ * unspecified.  Every valid output frame is what cmgan_tscnet_fwd computes for that utterance alone (same kernels, same order; only the
+ * order of the double-precision atomic additions of the InstanceNorm statistics may differ).  The workspace is
+ * cmgan_tscnet_workspace_bytes(B, T, F, precision): the same buffers as the uniform call.  Returns -1 when B * T * F * 320 >= 2^31 (the
+ * encoder's concat buffer is indexed with 32-bit element counts). */
+int cmgan_tscnet_fwd_ragged(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, const int* frames, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
 
 #ifdef __cplusplus
 }
