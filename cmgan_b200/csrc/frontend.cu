@@ -4,16 +4,66 @@
 //   the (1,2) output convolutions of both decoders (generator.py:126,150) and the final recombination
 //   (generator.py:136-139,188-196).  The framed DFT / inverse DFT themselves are GEMMs (gemm_args.h).
 #include "common.cuh"
+#include "frontend.cuh"
 #include "../../include/cmgan_b200.h"
 
 namespace {
 
 constexpr int NFFT = 400, HOP = 100, NF = 201;
 
+// ------------------------------------------------------------------ STFT tables
+// The window-folded DFT bases and the inverse overlap-add envelopes, built the way signal.py built them in torch float64 and rounded to
+// fp32 once: angle(r) = (2 pi r) / 400 with r = (n k) mod 400, window w[n] = 0.54 - 0.46 cos(angle(n)).  Every product, sum and quotient
+// is an explicit _rn intrinsic, so nvcc cannot contract a pair into an FMA: each step is the IEEE float64 operation torch performs, in
+// the same order, and only cos / sin of the 400 angles come from a different (device) libm.
+__device__ __forceinline__ double inv_envelope64(const double* w, int n, int T) {
+    const int p = n + NFFT / 2;                     // position in the un-trimmed envelope: sum_t w^2[p - 100 t], t increasing from 0.0
+    const int t_lo = p >= NFFT ? (p - NFFT) / HOP + 1 : 0, t_hi = min(p / HOP, T - 1);          // the frames that cover p
+    double e = 0.0;
+    for (int t = t_lo; t <= t_hi; ++t) {
+        const int m = p - t * HOP;
+        e = __dadd_rn(e, __dmul_rn(w[m], w[m]));
+    }
+    return __ddiv_rn(1.0, e);
+}
+
+__global__ void stft_tables_kernel(float* __restrict__ fwd, float* __restrict__ inv, int T, float* __restrict__ env, float* __restrict__ tail) {
+    __shared__ double cs[NFFT], sn[NFFT], w[NFFT];
+    for (int r = threadIdx.x; r < NFFT; r += blockDim.x) {
+        const double a = __ddiv_rn(__dmul_rn(2.0 * 3.141592653589793, (double)r), (double)NFFT);
+        cs[r] = cos(a);
+        sn[r] = sin(a);
+        w[r] = __dsub_rn(0.54, __dmul_rn(0.46, cs[r]));
+    }
+    __syncthreads();
+    const long nb = (long)NFFT * 2 * NF, nenv = env ? (long)HOP * (T - 1) : 0, total = 2 * nb + nenv + HOP;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        if (i < nb) {                               // fwd (400, 402): [w cos | -w sin]
+            if (!fwd) continue;
+            const int n = (int)(i / (2 * NF)), col = (int)(i % (2 * NF)), k = col < NF ? col : col - NF, r = n * k % NFFT;
+            fwd[i] = (float)(col < NF ? __dmul_rn(w[n], cs[r]) : __dmul_rn(-w[n], sn[r]));
+        } else if (i < 2 * nb) {                    // inv (402, 400): [wk cos w / 400 ; -wk sin w / 400], wk = 1, 2, ..., 2, 1
+            if (!inv) continue;
+            const long j = i - nb;
+            const int row = (int)(j / NFFT), n = (int)(j % NFFT), k = row < NF ? row : row - NF, r = n * k % NFFT;
+            const double wk = (k == 0 || k == NF - 1) ? 1.0 : 2.0;
+            const double v = row < NF ? __dmul_rn(__dmul_rn(wk, cs[r]), w[n]) : __dmul_rn(__dmul_rn(-wk, sn[r]), w[n]);
+            inv[j] = (float)__ddiv_rn(v, (double)NFFT);
+        } else if (i < 2 * nb + nenv) {             // 1 / envelope(T), n < 100 (T - 1)
+            const int n = (int)(i - 2 * nb);
+            env[n] = (float)inv_envelope64(w, n, T);
+        } else if (tail) {                          // the last 100 samples of 1 / envelope(T), any T >= 3: those of T = 8
+            const int n = (int)(i - 2 * nb - nenv);
+            tail[n] = (float)inv_envelope64(w, 6 * HOP + n, 8);
+        }
+    }
+}
+
 // ------------------------------------------------------------------ RMS scale: c[b] = sqrt(L / sum x^2)
-// RAGGED: row b has its own length lens[b] (clamped to [0, L])
+// RAGGED: row b has its own length lens[b] (clamped to [0, L]); tlen (optional) receives its frame count ceil(L_b / 100) + 1
 template <bool RAGGED>
-__global__ void rms_scale_kernel(const float* __restrict__ x, long ldx, int L, float* __restrict__ c, const int* __restrict__ lens) {
+__global__ void rms_scale_kernel(const float* __restrict__ x, long ldx, int L, float* __restrict__ c, const int* __restrict__ lens,
+                                 int* __restrict__ tlen) {
     __shared__ double sm[32];
     if (RAGGED) L = clamp_len(__ldg(lens + blockIdx.x), L);
     const float* p = x + (long)blockIdx.x * ldx;
@@ -26,6 +76,7 @@ __global__ void rms_scale_kernel(const float* __restrict__ x, long ldx, int L, f
         double t = 0.0;
         for (int w = 0; w < (blockDim.x >> 5); ++w) t += sm[w];
         c[blockIdx.x] = (float)sqrt((double)L / t);
+        if (RAGGED && tlen) tlen[blockIdx.x] = (L + HOP - 1) / HOP + 1;
     }
 }
 
@@ -48,23 +99,29 @@ __global__ void pad_reflect_kernel(const float* __restrict__ x, long ldx, int L,
 // with its own head to Lw = ceil(L_b / 100) * 100, reflect-padded by 200 on both sides and scaled by c[b]; zero from Lw + 400 up to Lp.
 // Needs L_b >= Lw - L_b and Lw > 200 (checked on the host); the value of every element is the one cmgan_pad_reflect gives the padded
 // utterance alone.
-__global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, const float* __restrict__ c,
-                                        float* __restrict__ xp, int Lp) {
+// FOLD (evaluation.py:25-34): every clip has L samples and lens is unused; clip b, wrap-padded to ceil(L / 100) * 100, is cut into k
+// segments of S = padded / k samples, and segment r becomes row b k + r, reflect-padded by 200 on each side (its own edges) and scaled by
+// c[b]: the rows signal.enhance feeds its DFT after the reshape, without the wrapped copy.  Needs S > 200 (checked on the host).
+template <bool FOLD>
+__global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, int k,
+                                        const float* __restrict__ c, float* __restrict__ xp, int Lp) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int b = blockIdx.y;
+    const int row = blockIdx.y;
     if (i >= Lp) return;
-    const int Lb = clamp_len(__ldg(lens + b), L);
-    const int Lw = (Lb + HOP - 1) / HOP * HOP;
+    const int b = FOLD ? row / k : row;
+    const int Lb = FOLD ? L : clamp_len(__ldg(lens + b), L);
+    const int Lw = FOLD ? (L + HOP - 1) / HOP * HOP / k : (Lb + HOP - 1) / HOP * HOP;        // FOLD: the segment length S
     float v = 0.f;
     if (Lb > 0 && i < Lw + NFFT) {
         int j = i - NFFT / 2;
         if (j < 0) j = -j;
         if (j >= Lw) j = 2 * (Lw - 1) - j;
+        if (FOLD) j += (row - b * k) * Lw;            // segment r starts at sample r S of the wrapped clip
         if (j >= Lb) j -= Lb;                         // wrap padding: sample Lb + k is sample k
         j = clamp_len(j, Lb - 1);                     // only reachable for lengths the host rejects
         v = __ldg(x + (long)b * ldx + j) * (c ? c[b] : 1.f);
     }
-    xp[(long)b * Lp + i] = v;
+    xp[(long)row * Lp + i] = v;
 }
 
 // S (B*T, 402) = [re | im]  ->  planes X[b, 0/1, t, f] = S * |S|^-0.7
@@ -154,8 +211,11 @@ __global__ void power_law_bwd_kernel(const float* __restrict__ re, const float* 
 }
 
 // overlap-add: y[b, n] = (sum_t frames[b, t, n + 200 - 100 t]) / env[n],  n < 100 (T - 1)
+// MAP (the folded clips of evaluation.py:30-34,52): row b is segment r = b % k of clip b / k; its samples go to y[b / k, r 100 (T - 1) + n]
+// below L (the reference's flatten()[:length]), de-normalised by c_div[b / k].  k = 1 writes y[b, n], n < L.
+template <bool MAP>
 __global__ void ola_kernel(const float* __restrict__ frames, int T, const float* __restrict__ inv_env, const float* __restrict__ c_div,
-                           float* __restrict__ y, long ldy) {
+                           float* __restrict__ y, long ldy, int k_seg, int L) {
     int n = blockIdx.x * blockDim.x + threadIdx.x;
     int b = blockIdx.y;
     int Lout = HOP * (T - 1);
@@ -169,6 +229,13 @@ __global__ void ola_kernel(const float* __restrict__ frames, int T, const float*
         if (k >= 0 && k < NFFT) s += __ldg(frames + ((long)b * T + t) * NFFT + k);
     }
     s *= inv_env[n];
+    if (MAP) {
+        const int clip = b / k_seg, o = (b - clip * k_seg) * Lout + n;
+        if (o >= L) return;
+        if (c_div) s /= c_div[clip];
+        y[(long)clip * ldy + o] = s;
+        return;
+    }
     if (c_div) s /= c_div[b];
     y[(long)b * ldy + n] = s;
 }
@@ -177,11 +244,15 @@ __global__ void ola_kernel(const float* __restrict__ frames, int T, const float*
 // with its own inverse envelope: 1 / envelope(T_b) equals inv_env (the table of the full T-frame grid) except over the last 100 samples,
 // where frame T_b is missing; there it is inv_tail[n - 100 (T_b - 2)], the same for every T_b >= 4 (signal._inv_envelope_tail).
 // Samples n >= 100 (T_b - 1) are written as zero.
+// MAP: y is the caller's (B, L) output; only the clip's own samples n < lens[b] (clamped to [0, L]) are written, nothing past them.
+template <bool MAP>
 __global__ void ola_ragged_kernel(const float* __restrict__ frames, int T, const int* __restrict__ tlen, const float* __restrict__ inv_env,
-                                  const float* __restrict__ inv_tail, const float* __restrict__ c_div, float* __restrict__ y, long ldy) {
+                                  const float* __restrict__ inv_tail, const float* __restrict__ c_div, float* __restrict__ y, long ldy,
+                                  const int* __restrict__ lens, int L) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
     if (n >= HOP * (T - 1)) return;
+    if (MAP && n >= clamp_len(__ldg(lens + b), L)) return;
     const int Tb = clamp_len(__ldg(tlen + b), T);
     const int Lout = HOP * (Tb - 1);
     float s = 0.f;
@@ -410,10 +481,53 @@ __global__ void recombine_bwd_kernel(const float* __restrict__ m1, MaskTail mt, 
 }  // namespace
 
 // ------------------------------------------------------------------ C ABI
+// any output may be null; inv_env (100 (T - 1) samples) needs T >= 2
+CMGAN_API int cmgan_stft_tables(float* fwd_basis, float* inv_basis, int T, float* inv_env, float* inv_tail, void* stream) {
+    CMGAN_REQUIRE(!inv_env || T >= 2, "cmgan_stft_tables: inv_env needs T >= 2 (T=%d)", T);
+    if (!fwd_basis && !inv_basis && !inv_env && !inv_tail) return 0;
+    stft_tables_kernel<<<128, 256, 0, (cudaStream_t)stream>>>(fwd_basis, inv_basis, T, inv_env, inv_tail);
+    return cmgan_check_launch("stft_tables_kernel");
+}
+
+int cmgan_rms_scale_frames(const float* x, long long ldx, int B, int L, const int* lengths, float* c, int* tlen, cudaStream_t st) {
+    CMGAN_REQUIRE(x && c && lengths && tlen && L > 0, "cmgan_rms_scale_frames: bad arguments");
+    if (B == 0) return 0;
+    rms_scale_kernel<true><<<B, 256, 0, st>>>(x, ldx, L, c, lengths, tlen);
+    return cmgan_check_launch("rms_scale_kernel");
+}
+
+int cmgan_pad_wrap_reflect_fold(const float* x, long long ldx, int B, int L, int k, const float* c, float* xp, int Lp, cudaStream_t st) {
+    const int S = (L + HOP - 1) / HOP * HOP / (k > 0 ? k : 1);
+    CMGAN_REQUIRE(x && xp && k > 0 && HOP % k == 0 && S > NFFT / 2 && Lp >= S + NFFT,
+                  "cmgan_pad_wrap_reflect_fold: need k | 100, S > 200 and Lp >= S + 400 (L=%d k=%d Lp=%d)", L, k, Lp);
+    if (B == 0) return 0;
+    dim3 grid(cdiv(Lp, 256), B * k);
+    pad_wrap_reflect_kernel<true><<<grid, 256, 0, st>>>(x, ldx, L, nullptr, k, c, xp, Lp);
+    return cmgan_check_launch("pad_wrap_reflect_kernel");
+}
+
+int cmgan_ola_fold(const float* frames, int rows, int T, int k, const float* inv_env, const float* c_div, float* y, long long ldy, int L,
+                   cudaStream_t st) {
+    CMGAN_REQUIRE(frames && inv_env && y && T >= 2 && k > 0 && rows % k == 0, "cmgan_ola_fold: bad arguments");
+    if (rows == 0) return 0;
+    dim3 grid(cdiv((long)HOP * (T - 1), 256), rows);
+    ola_kernel<true><<<grid, 256, 0, st>>>(frames, T, inv_env, c_div, y, ldy, k, L);
+    return cmgan_check_launch("ola_kernel");
+}
+
+int cmgan_ola_ragged_lengths(const float* frames, int B, int T, const int* tlen, const int* lengths, int L, const float* inv_env,
+                             const float* inv_tail, const float* c_div, float* y, long long ldy, cudaStream_t st) {
+    CMGAN_REQUIRE(frames && tlen && lengths && inv_env && inv_tail && y && T >= 2, "cmgan_ola_ragged_lengths: bad arguments");
+    if (B == 0) return 0;
+    dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
+    ola_ragged_kernel<true><<<grid, 256, 0, st>>>(frames, T, tlen, inv_env, inv_tail, c_div, y, ldy, lengths, L);
+    return cmgan_check_launch("ola_ragged_kernel");
+}
+
 CMGAN_API int cmgan_rms_scale(const float* x, long long ldx, int B, int L, float* c, void* stream) {
     CMGAN_REQUIRE(x && c && L > 0, "cmgan_rms_scale: bad arguments");
     if (B == 0) return 0;
-    rms_scale_kernel<false><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, nullptr);
+    rms_scale_kernel<false><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, nullptr, nullptr);
     return cmgan_check_launch("rms_scale_kernel");
 }
 
@@ -421,7 +535,7 @@ CMGAN_API int cmgan_rms_scale(const float* x, long long ldx, int B, int L, float
 CMGAN_API int cmgan_rms_scale_ragged(const float* x, long long ldx, int B, int L, const int* lengths, float* c, void* stream) {
     CMGAN_REQUIRE(x && c && lengths && L > 0, "cmgan_rms_scale_ragged: bad arguments");
     if (B == 0) return 0;
-    rms_scale_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, lengths);
+    rms_scale_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, lengths, nullptr);
     return cmgan_check_launch("rms_scale_kernel");
 }
 
@@ -433,7 +547,7 @@ CMGAN_API int cmgan_pad_wrap_reflect_ragged(const float* x, long long ldx, int B
                   "cmgan_pad_wrap_reflect_ragged: need Lp >= ceil(L / 100) * 100 + 400 (L=%d Lp=%d)", L, Lp);
     if (B == 0) return 0;
     dim3 grid(cdiv(Lp, 256), B);
-    pad_wrap_reflect_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, c, xp, Lp);
+    pad_wrap_reflect_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, 1, c, xp, Lp);
     return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 
@@ -475,7 +589,7 @@ CMGAN_API int cmgan_ola(const float* frames, int B, int T, const float* inv_env,
     CMGAN_REQUIRE(frames && inv_env && y && T >= 2, "cmgan_ola: bad arguments");
     if (B == 0) return 0;
     dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
-    ola_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, inv_env, c_div, y, ldy);
+    ola_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, inv_env, c_div, y, ldy, 1, 0);
     return cmgan_check_launch("ola_kernel");
 }
 
@@ -484,7 +598,7 @@ CMGAN_API int cmgan_ola_ragged(const float* frames, int B, int T, const int* tle
     CMGAN_REQUIRE(frames && tlen && inv_env && inv_tail && y && T >= 2, "cmgan_ola_ragged: bad arguments");
     if (B == 0) return 0;
     dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
-    ola_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, tlen, inv_env, inv_tail, c_div, y, ldy);
+    ola_ragged_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, tlen, inv_env, inv_tail, c_div, y, ldy, nullptr, 0);
     return cmgan_check_launch("ola_ragged_kernel");
 }
 

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "frontend.cuh"
 #include "../../include/cmgan_b200.h"
 
 namespace {
@@ -355,6 +356,86 @@ void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt
     if ((size_t)(sums - sums0) > n_sums && r.rc == 0) { cmgan_set_error("cmgan_tscnet_fwd: statistics scratch exhausted"); r.rc = -1; }
 }
 
+// ---- waveform in, waveform out (evaluation.py:21-53): the launch sequence of signal.enhance / enhance_ragged around forward()
+constexpr int NFFT = 400, HOP = 100;
+
+struct EnhanceGeom { int k, S, T, Lp, rows; };
+
+// evaluation.py:25-34: wrap padding to padded = ceil(L / 100) * 100; past cut_len the clip is folded into k segments of S = padded / k
+// samples, k = ceil(padded / cut_len) raised until it divides 100.  0, or -1 with the message set.
+int enhance_geom(int B, int L, int cut_len, bool ragged, EnhanceGeom& g, const char* who) {
+    CMGAN_REQUIRE(B > 0, "%s: B must be positive (B=%d)", who, B);
+    CMGAN_REQUIRE(L > NFFT / 2, "%s: L=%d samples; a clip needs more than the 200-sample reflect padding of the STFT", who, L);
+    CMGAN_REQUIRE(cut_len > 0, "%s: cut_len must be positive (cut_len=%d)", who, cut_len);
+    const long long padded = ((long long)L + HOP - 1) / HOP * HOP;
+    CMGAN_REQUIRE(padded - L <= L, "%s: wrap padding L=%d to %lld is longer than the clip", who, L, padded);
+    long long k = 1;
+    if (padded > cut_len) {
+        CMGAN_REQUIRE(!ragged, "%s: a ragged batch needs ceil(L / 100) * 100 <= cut_len (L=%d, cut_len=%d); longer clips take the uniform call, "
+                      "which folds them", who, L, cut_len);
+        k = (padded + cut_len - 1) / cut_len;
+        while (k <= HOP && HOP % k != 0) ++k;
+        CMGAN_REQUIRE(k <= HOP, "%s: L=%d with cut_len=%d folds into more than 100 segments", who, L, cut_len);
+    }
+    g.k = (int)k;
+    g.S = (int)(padded / k);
+    CMGAN_REQUIRE(g.S > NFFT / 2, "%s: L=%d with cut_len=%d folds into %d segments of %d samples; a segment needs more than 200", who, L,
+                  cut_len, g.k, g.S);
+    g.T = g.S / HOP + 1;
+    CMGAN_REQUIRE(k * HOP * (g.T - 1) >= L, "%s: L=%d with cut_len=%d folds into %d segments of %d samples, which yield only %lld samples", who,
+                  L, cut_len, g.k, g.S, k * HOP * (g.T - 1));
+    const long long elems = (long long)B * k * g.T * NFEAT * CAT;
+    CMGAN_REQUIRE(elems < (1ll << 31), "%s: rows * T * 201 * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split "
+                  "the batch", who, CAT, elems);
+    g.rows = (int)(B * k);
+    g.Lp = (g.S + NFFT + HOP - 1) / HOP * HOP;
+    return 0;
+}
+
+void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const int* lengths, const EnhanceGeom& g, float* out, long long ldo) {
+    const int T = g.T, rows = g.rows, F = NFEAT;
+    const long long MT = (long long)rows * T;
+    float* fwd = r.alloc((size_t)NFFT * 2 * F);
+    float* inv = r.alloc((size_t)2 * F * NFFT);
+    float* env = r.alloc((size_t)HOP * (T - 1));
+    float* tail = r.alloc(HOP);
+    float* c = r.alloc(B);
+    int* tlen = r.alloc<int>(B);
+    float* X = r.alloc((size_t)MT * 2 * F);
+    float* fr = r.alloc((size_t)MT * F);
+    float* fi = r.alloc((size_t)MT * F);
+    if (r.live()) r.ok(cmgan_stft_tables(fwd, inv, T, env, tail, r.st));
+    if (r.live()) r.ok(lengths ? cmgan_rms_scale_frames(wav, ldw, B, L, lengths, c, tlen, r.st) : cmgan_rms_scale(wav, ldw, B, L, c, r.st));
+    const size_t mark = r.top;
+    // ---- signal._stft_padded: wrap + reflect (+ fold) padding, framed DFT (exact fp32 FFMA), power compression
+    {
+        float* xp = r.alloc((size_t)rows * g.Lp);
+        float* S = r.alloc((size_t)MT * 2 * F);
+        if (r.live())
+            r.ok(lengths ? cmgan_pad_wrap_reflect_ragged(wav, ldw, B, L, lengths, c, xp, g.Lp, r.st)
+                         : cmgan_pad_wrap_reflect_fold(wav, ldw, B, L, g.k, c, xp, g.Lp, r.st));
+        Gemm dft(xp, HOP, fwd, 0, 2 * F, 1, nullptr, S, 2 * F, MT, 2 * F, NFFT);
+        dft.conv(1, T, 1, g.Lp / HOP);
+        if (r.live()) r.ok(cmgan_gemm_rows_f32(&dft.a, r.st));          // precision 0 (memset by Gemm): the DFTs stay exact fp32
+        if (r.live()) r.ok(cmgan_compress(S, rows, T, X, r.st));
+        r.top = mark;
+    }
+    // ---- TSCNet.forward on (rows, 2, T, F) contiguous; a ragged batch passes its frame counts
+    r.frames = lengths ? tlen : nullptr;
+    forward(r, X, 2LL * T * F, (long long)T * F, F, 1, rows, T, F, fr, fi);
+    r.frames = nullptr;
+    r.top = mark;
+    // ---- signal.uncompress_istft_fwd: un-compression, inverse DFT (exact fp32 FFMA), overlap-add straight into `out`
+    float* U = r.alloc((size_t)MT * 2 * F);
+    float* frames = r.alloc((size_t)MT * NFFT);
+    if (r.live()) r.ok(cmgan_uncompress(fr, fi, (long long)T * F, F, 1, rows, T, U, r.st));
+    Gemm idft(U, 2 * F, inv, 0, NFFT, 1, nullptr, frames, NFFT, MT, NFFT, 2 * F);
+    if (r.live()) r.ok(cmgan_gemm_rows_f32(&idft.a, r.st));
+    if (r.live())
+        r.ok(lengths ? cmgan_ola_ragged_lengths(frames, B, T, tlen, lengths, L, env, tail, c, out, ldo, r.st)
+                     : cmgan_ola_fold(frames, rows, T, g.k, env, c, out, ldo, L, r.st));
+}
+
 }  // namespace
 
 CMGAN_API int cmgan_tscnet_param_count(void) { return (int)table().e.size(); }
@@ -407,4 +488,39 @@ CMGAN_API int cmgan_tscnet_fwd_ragged(const float* params, const float* x, long 
                   "cmgan_tscnet_fwd_ragged: B * T * F * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split the batch",
                   CAT, (long long)B * T * F * CAT);
     return tscnet_fwd(params, x, sxb, sxc, sxt, sxf, B, T, F, frames, final_real, final_imag, workspace, workspace_bytes, precision, stream);
+}
+
+// one size for the uniform and the ragged call at (B, L, cut_len): the walk allocates the same buffers in both modes
+static long long enhance_bytes(int B, int L, const EnhanceGeom& g, int precision) {
+    Run r;
+    r.P = nullptr; r.ws = nullptr; r.dry = true; r.precision = precision; r.st = nullptr;
+    enhance_walk(r, nullptr, L, B, L, nullptr, g, nullptr, L);
+    return (long long)r.peak + 256;
+}
+
+CMGAN_API long long cmgan_enhance_workspace_bytes(int B, int L, int cut_len, int precision) {
+    if (precision != 0 && precision != 1) { cmgan_set_error("cmgan_enhance_workspace_bytes: precision must be 0 (fp32) or 1 (tf32)"); return -1; }
+    EnhanceGeom g;
+    if (enhance_geom(B, L, cut_len, false, g, "cmgan_enhance_workspace_bytes") != 0) return -1;
+    return enhance_bytes(B, L, g, precision);
+}
+
+CMGAN_API int cmgan_enhance(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int cut_len, float* out,
+                            long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream) {
+    CMGAN_REQUIRE(params && wav && out && workspace, "cmgan_enhance: null pointer");
+    CMGAN_REQUIRE(precision == 0 || precision == 1, "cmgan_enhance: precision must be 0 (fp32) or 1 (tf32)");
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "cmgan_enhance: params must be 16-byte, workspace 256-byte aligned");
+    EnhanceGeom g;
+    if (enhance_geom(B, L, cut_len, lengths != nullptr, g, "cmgan_enhance") != 0) return -1;
+    CMGAN_REQUIRE(ldw >= L && ldo >= L, "cmgan_enhance: row strides must cover a clip (L=%d ldw=%lld ldo=%lld)", L, ldw, ldo);
+    const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + (B - 1) * ldw + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + (B - 1) * ldo + L);
+    CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "cmgan_enhance: wav and out overlap");
+    const long long need = enhance_bytes(B, L, g, precision);
+    CMGAN_REQUIRE(workspace_bytes >= need, "cmgan_enhance: workspace too small (%lld bytes needed, %lld given)", need, workspace_bytes);
+    cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
+    Run r;
+    r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
+    r.st = (cudaStream_t)stream;
+    enhance_walk(r, wav, ldw, B, L, lengths, g, out, ldo);
+    return r.rc;
 }

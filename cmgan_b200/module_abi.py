@@ -1,7 +1,8 @@
 """Python view of the module-level C entry points (``cmgan_tscnet_*`` in include/cmgan_b200.h): the same calls a C / C++ host makes.
 
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
-workspace; torch is used here only to own the device memory."""
+workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
+out.  torch is used here only to own the device memory."""
 from __future__ import annotations
 
 import ctypes
@@ -61,3 +62,33 @@ def tscnet_forward(flat: torch.Tensor, x: torch.Tensor, precision: int = 1, work
         lib().call("cmgan_tscnet_fwd_ragged", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, fdev.data_ptr(), fr.data_ptr(), fi.data_ptr(),
                    workspace.data_ptr(), workspace.numel(), precision, stream)
     return fr, fi
+
+
+def enhance_workspace_bytes(B: int, L: int, cut_len: int = 16000 * 16, precision: int = 1) -> int:
+    """workspace of ``cmgan_enhance`` for B clips of up to L samples (the same size for the uniform and the ragged call)"""
+    n = lib().cdll.cmgan_enhance_workspace_bytes(B, L, cut_len, precision)
+    if n < 0:
+        raise RuntimeError(lib().cdll.cmgan_last_error().decode())
+    return n
+
+
+def enhance(flat: torch.Tensor, wav: torch.Tensor, lengths=None, cut_len: int = 16000 * 16, precision: int = 1, workspace: torch.Tensor = None,
+            out: torch.Tensor = None) -> torch.Tensor:
+    """``cmgan_enhance``: noisy waveforms (B, L) on the GPU (unit row stride) -> enhanced waveforms in ``out`` (B, L), which is returned.
+    ``lengths=None``: every row is a clip of L samples (folded past ``cut_len``, as evaluation.py does).  Otherwise a ragged batch: clip b is
+    wav[b, :lengths[b]] (a device int32 (B,) tensor is used as is, anything else goes through torch.as_tensor); out[b, lengths[b]:] is left
+    as it was (zeros when ``out`` is allocated here)."""
+    assert wav.is_cuda and flat.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
+    B, L = wav.shape
+    if workspace is None:
+        workspace = torch.empty(enhance_workspace_bytes(B, L, cut_len, precision), dtype=torch.uint8, device=wav.device)
+    if out is None:
+        out = (torch.empty if lengths is None else torch.zeros)(B, L, device=wav.device)
+    assert out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (B, L) and out.stride(1) == 1
+    lens = None
+    if lengths is not None:
+        lens = torch.as_tensor(lengths, dtype=torch.int32, device=wav.device).reshape(-1).contiguous()
+        assert lens.numel() == B, f"lengths has {lens.numel()} entries for a batch of {B}"
+    lib().call("cmgan_enhance", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), cut_len,
+               out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    return out

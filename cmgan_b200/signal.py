@@ -18,59 +18,36 @@ N_FFT, HOP, NF = 400, 100, 201
 _CACHE: Dict[Tuple, torch.Tensor] = {}
 
 
-def _window64():
-    k = torch.arange(N_FFT, dtype=torch.float64)
-    return 0.54 - 0.46 * torch.cos(2.0 * math.pi * k / N_FFT)
+def _table(key, shape, fill) -> torch.Tensor:
+    """per-device cache of one STFT table, filled by ``cmgan_stft_tables`` (float64 on the device, rounded to fp32 once): the tables the
+    C entry ``cmgan_enhance`` builds in its workspace, bit for bit"""
+    if key not in _CACHE:
+        t = torch.empty(shape, dtype=torch.float32, device=key[-1])
+        with torch.cuda.device(t.device):
+            fill(t)
+        _CACHE[key] = t
+    return _CACHE[key]
 
 
 def _fwd_basis(dev) -> torch.Tensor:
-    """(400, 402): [w[n] cos(2 pi k n / 400) | -w[n] sin(2 pi k n / 400)], generated in float64"""
-    key = ("fwd", dev)
-    if key not in _CACHE:
-        n = torch.arange(N_FFT, dtype=torch.float64).unsqueeze(1)
-        k = torch.arange(NF, dtype=torch.float64).unsqueeze(0)
-        ang = 2.0 * math.pi * torch.remainder(n * k, N_FFT) / N_FFT
-        w = _window64().unsqueeze(1)
-        _CACHE[key] = torch.cat([w * torch.cos(ang), -w * torch.sin(ang)], dim=1).to(torch.float32).contiguous().to(dev)
-    return _CACHE[key]
+    """(400, 402): [w[n] cos(2 pi k n / 400) | -w[n] sin(2 pi k n / 400)], w the periodic Hamming window"""
+    return _table(("fwd", dev), (N_FFT, 2 * NF), lambda t: call("cmgan_stft_tables", t, None, 0, None, None))
 
 
 def _inv_basis(dev) -> torch.Tensor:
     """(402, 400): one-sided inverse DFT (weights 1, 2, ..., 2, 1; /400) times the synthesis window"""
-    key = ("inv", dev)
-    if key not in _CACHE:
-        n = torch.arange(N_FFT, dtype=torch.float64).unsqueeze(0)
-        k = torch.arange(NF, dtype=torch.float64).unsqueeze(1)
-        ang = 2.0 * math.pi * torch.remainder(k * n, N_FFT) / N_FFT
-        wk = torch.full((NF, 1), 2.0, dtype=torch.float64)
-        wk[0, 0] = 1.0
-        wk[NF - 1, 0] = 1.0
-        w = _window64().unsqueeze(0)
-        _CACHE[key] = torch.cat([wk * torch.cos(ang) * w / N_FFT, -wk * torch.sin(ang) * w / N_FFT], dim=0).to(torch.float32).contiguous().to(dev)
-    return _CACHE[key]
+    return _table(("inv", dev), (2 * NF, N_FFT), lambda t: call("cmgan_stft_tables", None, t, 0, None, None))
 
 
 def _inv_envelope(T: int, dev) -> torch.Tensor:
     """1 / sum_t w^2[n + 200 - 100 t] for n < 100 (T - 1)"""
-    key = ("env", T, dev)
-    if key not in _CACHE:
-        w2 = _window64() ** 2
-        out_len = N_FFT + HOP * (T - 1)
-        env = torch.zeros(out_len, dtype=torch.float64)
-        for t in range(T):
-            env[t * HOP:t * HOP + N_FFT] += w2
-        env = env[N_FFT // 2: out_len - N_FFT // 2]
-        _CACHE[key] = (1.0 / env).to(torch.float32).contiguous().to(dev)
-    return _CACHE[key]
+    return _table(("env", T, dev), (HOP * (T - 1),), lambda t: call("cmgan_stft_tables", None, None, T, t, None))
 
 
 def _inv_envelope_tail(dev) -> torch.Tensor:
     """the last 100 samples of 1 / envelope(T), the same for every T >= 3: at n >= 100 (T - 2) frame T is missing, elsewhere envelope(T)
     equals envelope(T') for any T' >= T (the ragged overlap-add combines this tail with the table of the longest utterance)"""
-    key = ("env_tail", dev)
-    if key not in _CACHE:
-        _CACHE[key] = _inv_envelope(8, dev)[600:700].contiguous()
-    return _CACHE[key]
+    return _table(("env_tail", dev), (HOP,), lambda t: call("cmgan_stft_tables", None, None, 0, None, t))
 
 
 def rms_scale(wav: torch.Tensor) -> torch.Tensor:

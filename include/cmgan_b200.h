@@ -82,6 +82,10 @@ int cmgan_power_law_bwd(const float* re, const float* im, long long i0, long lon
 int cmgan_ola(const float* frames, int B, int T, const float* inv_env, const float* c_div, float* y, long long ldy, void* stream);
 int cmgan_ola_ragged(const float* frames, int B, int T, const int* tlen, const float* inv_env, const float* inv_tail, const float* c_div, float* y, long long ldy, void* stream);
 int cmgan_ola_bwd(const float* dy, long long lddy, int B, int T, const float* inv_env, float* dframes, void* stream);
+/* STFT tables (n_fft 400, hop 100, periodic Hamming), built on the device from float64 arithmetic and rounded to fp32 once; any output may
+ * be null.  fwd_basis (400, 402) = [w cos | -w sin]; inv_basis (402, 400) = the one-sided inverse DFT (weights 1, 2, ..., 2, 1; / 400) times
+ * the window; inv_env = 1 / overlap-add envelope of T >= 2 frames (100 (T - 1) samples); inv_tail = its last 100 samples for any T >= 3. */
+int cmgan_stft_tables(float* fwd_basis, float* inv_basis, int T, float* inv_env, float* inv_tail, void* stream);
 
 /* ---- generator head and tails (generator.py:53,126,136-139,150,175-196) */
 int cmgan_head_conv(const float* x, long long sb, long long sc, long long st, long long sf, int B, int T, int F, const float* w, const float* bias, float* out, long long ldo, void* stream);
@@ -137,6 +141,23 @@ int cmgan_tscnet_fwd(const float* params, const float* x, long long sxb, long lo
  * cmgan_tscnet_workspace_bytes(B, T, F, precision): the same buffers as the uniform call.  Returns -1 when B * T * F * 320 >= 2^31 (the
  * encoder's concat buffer is indexed with 32-bit element counts). */
 int cmgan_tscnet_fwd_ragged(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, const int* frames, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
+
+/* ---- module level, waveform in / waveform out: evaluation.py:21-53 (enhance_one_track between load and save) as one call.
+ * wav (B, L) fp32 with row stride ldw; out (B, L) fp32 with row stride ldo; neither range may overlap the other.  Per clip: RMS scale,
+ * wrap padding to a multiple of 100, the STFT, power compression, TSCNet.forward (params / precision as cmgan_tscnet_fwd), un-compression,
+ * the inverse STFT, de-normalisation, truncation to the clip's length.  Each clip gets what it would get enhanced alone.
+ *   lengths == NULL: B clips of exactly L samples.  A clip whose padded length exceeds cut_len is folded into k segments as the reference
+ *     does (k = ceil(padded / cut_len), raised until it divides 100); every out[b, :L] is written.
+ *   lengths != NULL: device int32[B], clip b is wav[b, :lengths[b]] (values clamped to [0, L] on the device); wav[b, n >= len_b] is never
+ *     read and out[b, n >= len_b] never written.  Needs ceil(L / 100) * 100 <= cut_len (longer clips take the uniform, folding call).  Every
+ *     length must satisfy the wrap-padding precondition: padded_b = ceil(len_b / 100) * 100 > 200 and padded_b - len_b <= len_b (any
+ *     len_b >= 201 does).  A clip that breaks it gets an unspecified output; nothing out of bounds is touched.
+ * The workspace (256-byte aligned) holds the STFT tables, regenerated on every call, and every intermediate; cmgan_enhance_workspace_bytes
+ * sizes it for both modes and returns -1 (message in cmgan_last_error) for any shape cmgan_enhance rejects: B <= 0, L <= 200, a folded
+ * segment of 200 samples or fewer, a fold that yields fewer than L samples, or rows * T * 201 * 320 >= 2^31 (rows = B, or B k folded; T =
+ * segment length / 100 + 1 frames).  Allocates nothing, never synchronises, CUDA-graph capturable. */
+long long cmgan_enhance_workspace_bytes(int B, int L, int cut_len, int precision);
+int cmgan_enhance(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int cut_len, float* out, long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream);
 
 #ifdef __cplusplus
 }
