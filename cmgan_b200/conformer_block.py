@@ -250,7 +250,11 @@ def conformer_bwd(dy, S: dict, P, G: Dict[str, torch.Tensor], B, T, F2, sums: _S
     # ---- convolution module: x3 = x2 + W7 swish(bn(d)) + b7
     bn = S["bn"]
     dbn = _empty(M, 2 * C, dev=dev)
-    gemm(A=dx3, lda=C, W=P[f"{p}.conv.net.7.weight"], sb_k=2 * C, sb_n=1, C=dbn, ldc=2 * C, M=M, N=2 * C, Cin=C, epi=EPI_DBNSWISH, aux=S["d"],
+    dx3_op = dx3
+    if ops.PRECISION == 1:      # dx3 also carries the residual gradient at full precision: the tensor-core operand is a rounded copy
+        dx3_op = _empty(M, C, dev=dev)
+        call("cmgan_copy_rows_operand", dx3, C, dx3_op, C, M, C)
+    gemm(A=dx3_op, lda=C, W=P[f"{p}.conv.net.7.weight"], sb_k=2 * C, sb_n=1, C=dbn, ldc=2 * C, M=M, N=2 * C, Cin=C, epi=EPI_DBNSWISH, aux=S["d"],
          ldaux=2 * C, e0=bn.scale, e1=bn.shift)
     gemm(wgrad=True, A=S["dsw"], lda=2 * C, Cin=2 * C, D=dx3, ldd=C, N=C, W=None, C=G[f"{p}.conv.net.7.weight"], sb_k=1, sb_n=2 * C, ldc=0, M=M,
          dbias=G[f"{p}.conv.net.7.bias"])
