@@ -478,6 +478,127 @@ __global__ void recombine_bwd_kernel(const float* __restrict__ m1, MaskTail mt, 
     if ((threadIdx.x & 31) == 0) { atomicAdd(dfcw, pw); atomicAdd(dfcb, pb); }
 }
 
+// ------------------------------------------------------------------ input gradients (differentiable front end)
+// *dst += sum of v over the block (blockDim.x a multiple of 32, at most 1024); every thread of the block must call it
+__device__ __forceinline__ void block_sum_atomic(float v, float* dst) {
+    __shared__ float sm[32];
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sm[w];
+        atomicAdd(dst, s);
+    }
+}
+
+// gradient of TSCNet wrt its input x (B, 2, T, F).  final = mask x + cplx (recombine_kernel) and the head convolution reads [|x|, re, im]
+// (head_conv_kernel), so with draw = the gradient of the raw head output (rows m, 64 channels) and w the head weight (64, 3):
+//   dre = mask dfr + sum_n draw[m, n] (w[n, 1] + w[n, 0] re / |x|),   dim = mask dfi + sum_n draw[m, n] (w[n, 2] + w[n, 0] im / |x|).
+// At |x| = 0 the magnitude term contributes 0 (the reference's autograd gives NaN there: the derivative of sqrt at 0).  The mask is
+// recomputed from m1 as recombine_bwd_kernel does.  16 threads per row, 4 channels each; dx is contiguous (B, 2, T, F).
+__global__ void tscnet_input_grad_kernel(const float* __restrict__ m1, MaskTail mt, const float* __restrict__ x, long sb, long sc, long st,
+                                         long sf, const float* __restrict__ dfr, const float* __restrict__ dfi, long gb, long gt, long gf,
+                                         const float* __restrict__ draw, long ldd, const float* __restrict__ w, int T, int F, long M,
+                                         float* __restrict__ dx) {
+    const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long m = idx >> 4;
+    const int c4 = (int)(idx & 15) * 4;
+    float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+    if (m < M) {
+        const float4 d = __ldg(reinterpret_cast<const float4*>(draw + m * ldd + c4));
+        const float dv[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = c4 + j;
+            s0 = fmaf(dv[j], __ldg(w + n * 3), s0);
+            s1 = fmaf(dv[j], __ldg(w + n * 3 + 1), s1);
+            s2 = fmaf(dv[j], __ldg(w + n * 3 + 2), s2);
+        }
+    }
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) {           // the 16 threads of a row are 16 consecutive lanes
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if (m >= M || c4 != 0) return;
+    const int f = (int)(m % F); const long bt = m / F; const int t = (int)(bt % T); const long b = bt / T;
+    float z = __ldg(m1 + m) * mt.scale[b] + mt.shift[b];
+    if (z < 0.f) z *= mt.a1[0];
+    const float z2 = fmaf(mt.fcw[0], z, mt.fcb[0]);
+    const float mask = z2 >= 0.f ? z2 : z2 * __ldg(mt.slope_f + f);
+    const long o = b * sb + t * st + f * sf;
+    const float re = __ldg(x + o), im = __ldg(x + o + sc);
+    const float mag = sqrtf(re * re + im * im);
+    const float sm = mag > 0.f ? s0 / mag : 0.f;
+    const long go = b * gb + t * gt + f * gf;
+    const long q = ((b * 2) * T + t) * F + f;
+    dx[q] = fmaf(mask, __ldg(dfr + go), fmaf(sm, re, s1));
+    dx[q + (long)T * F] = fmaf(mask, __ldg(dfi + go), fmaf(sm, im, s2));
+}
+
+// gradient of c[b] = sqrt(L / sum x^2):  dc / dx_i = -c^3 x_i / L,  dx[b, i] (+)= -dc[b] c[b]^3 x[b, i] / L
+__global__ void rms_scale_bwd_kernel(const float* __restrict__ x, long ldx, int L, const float* __restrict__ c, const float* __restrict__ dc,
+                                     float* __restrict__ dx, long lddx, int accumulate) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (i >= L) return;
+    const float cb = c[b];
+    const float k = -dc[b] * cb * cb * cb / (float)L;
+    const float v = k * __ldg(x + (long)b * ldx + i);
+    float* p = dx + (long)b * lddx + i;
+    *p = accumulate ? *p + v : v;
+}
+
+// adjoint of the framing + reflect padding + scaling in front of the DFT (pad_reflect_kernel, frame t = xp[100 t, 100 t + 400)).
+// dframes (B*T, 400) -> g[b, j] = sum over the padded positions p that read x[b, j] (p = j + 200, p = 200 - j for j <= 200, p = 2 (L - 1) - j
+// + 200 for j >= L - 201) of sum over the frames t that cover p of dframes[b, t, p - 100 t];  dx[b, j] = c[b] g[b, j] (c null: 1) and
+// dc[b] += sum_j g[b, j] x[b, j] (dc optional, zeroed by the caller).  Needs L > 200 (one reflection per side) and T = L / 100 + 1.
+__device__ __forceinline__ float frames_at(const float* __restrict__ df, int T, int p) {
+    const int t_lo = p >= NFFT ? (p - NFFT) / HOP + 1 : 0, t_hi = min(p / HOP, T - 1);
+    float s = 0.f;
+    for (int t = t_lo; t <= t_hi; ++t) s += __ldg(df + (long)t * NFFT + p - t * HOP);
+    return s;
+}
+
+__global__ void pad_reflect_bwd_kernel(const float* __restrict__ dframes, int T, const float* __restrict__ x, long ldx, int L,
+                                       const float* __restrict__ c, float* __restrict__ dx, long lddx, float* __restrict__ dc) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    const float* df = dframes + (long)b * T * NFFT;
+    float gx = 0.f;
+    if (j < L) {
+        float g = frames_at(df, T, j + NFFT / 2);
+        if (j >= 1 && j <= NFFT / 2) g += frames_at(df, T, NFFT / 2 - j);
+        if (j >= L - 1 - NFFT / 2 && j <= L - 2) g += frames_at(df, T, 2 * (L - 1) - j + NFFT / 2);
+        dx[(long)b * lddx + j] = c ? c[b] * g : g;
+        gx = g * __ldg(x + (long)b * ldx + j);
+    }
+    if (dc) block_sum_atomic(gx, dc + b);
+}
+
+// gradient of the de-normalised overlap-add y = ola(frames) / c_div (ola_kernel with c_div): dframes[b, t, k] = dy[b, n] inv_env[n] / c_div[b]
+// (n = 100 t + k - 200, zero outside the trimmed range) and dc[b] += -sum_n dy[b, n] y[b, n] / c_div[b] (dc optional, zeroed by the caller)
+__global__ void ola_div_bwd_kernel(const float* __restrict__ dy, long lddy, int T, const float* __restrict__ inv_env, const float* __restrict__ c_div,
+                                   const float* __restrict__ y, long ldy, float* __restrict__ dframes, float* __restrict__ dc) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    const int Lout = HOP * (T - 1);
+    const float cb = c_div[b];
+    if (i < (long)T * NFFT) {
+        const int t = (int)(i / NFFT), k = (int)(i % NFFT);
+        const int n = t * HOP + k - NFFT / 2;
+        float v = 0.f;
+        if (n >= 0 && n < Lout) v = __ldg(dy + (long)b * lddy + n) * inv_env[n] / cb;
+        dframes[(long)b * T * NFFT + i] = v;
+    }
+    if (dc) {
+        const float p = i < Lout ? __ldg(dy + (long)b * lddy + i) * __ldg(y + (long)b * ldy + i) : 0.f;
+        block_sum_atomic(-p / cb, dc + b);
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------ C ABI
@@ -693,4 +814,61 @@ CMGAN_API int cmgan_power_law_bwd(const float* re, const float* im, long long i0
     if (n == 0) return 0;
     power_law_bwd_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(re, im, i0, i1, i2, gre, gim, o0, o1, o2, dre, dim_, q0, q1, q2, d1, d2, n, p);
     return cmgan_check_launch("power_law_bwd_kernel");
+}
+
+// ------------------------------------------------------------------ input gradients (differentiable front end)
+// dx (B, 2, T, F) contiguous = the gradient of TSCNet wrt its input x (see tscnet_input_grad_kernel); draw (M, ldd) 16-byte aligned, ldd % 4 == 0
+CMGAN_API int cmgan_tscnet_input_grad(const float* m1, const float* in_scale, const float* in_shift, const float* a1, const float* fcw,
+                                      const float* fcb, const float* slope_f, const float* x, long long sb, long long sc, long long st,
+                                      long long sf, const float* dfr, const float* dfi, long long gb, long long gt, long long gf,
+                                      const float* draw, long long ldd, const float* w, int B, int T, int F, float* dx, void* stream) {
+    CMGAN_REQUIRE(m1 && in_scale && in_shift && a1 && fcw && fcb && slope_f && x && dfr && dfi && draw && w && dx,
+                  "cmgan_tscnet_input_grad: null pointer");
+    CMGAN_REQUIRE(ldd >= 64 && ldd % 4 == 0 && ((uintptr_t)draw & 15) == 0,
+                  "cmgan_tscnet_input_grad: draw needs 16-byte alignment and ldd >= 64, ldd %% 4 == 0 (ldd=%lld)", ldd);
+    CMGAN_REQUIRE(B >= 0 && T >= 0 && F >= 0, "cmgan_tscnet_input_grad: negative size (B=%d T=%d F=%d)", B, T, F);
+    const long M = (long)B * T * F;
+    if (M == 0) return 0;
+    MaskTail mt{in_scale, in_shift, a1, fcw, fcb, slope_f};
+    tscnet_input_grad_kernel<<<cdiv(M * 16, 256), 256, 0, (cudaStream_t)stream>>>(m1, mt, x, sb, sc, st, sf, dfr, dfi, gb, gt, gf, draw, ldd, w,
+                                                                                  T, F, M, dx);
+    return cmgan_check_launch("tscnet_input_grad_kernel");
+}
+
+// dx[b, i] (+)= -dc[b] c[b]^3 x[b, i] / L: the gradient of cmgan_rms_scale
+CMGAN_API int cmgan_rms_scale_bwd(const float* x, long long ldx, int B, int L, const float* c, const float* dc, float* dx, long long lddx,
+                                  int accumulate, void* stream) {
+    CMGAN_REQUIRE(x && c && dc && dx, "cmgan_rms_scale_bwd: null pointer");
+    CMGAN_REQUIRE(B >= 0 && L > 0 && ldx >= L && lddx >= L, "cmgan_rms_scale_bwd: need L > 0 and row strides >= L (L=%d ldx=%lld lddx=%lld)",
+                  L, ldx, lddx);
+    if (B == 0) return 0;
+    dim3 grid(cdiv(L, 256), B);
+    rms_scale_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, c, dc, dx, lddx, accumulate);
+    return cmgan_check_launch("rms_scale_bwd_kernel");
+}
+
+// adjoint of cmgan_pad_reflect + the framing of the DFT: dframes (B*T, 400), T = L / 100 + 1 -> dx (B, L) = c g (c may be null: 1) and
+// dc[b] += sum_j g[b, j] x[b, j] (dc may be null; the caller zeroes it)
+CMGAN_API int cmgan_pad_reflect_bwd(const float* dframes, int B, int T, const float* x, long long ldx, int L, const float* c, float* dx,
+                                    long long lddx, float* dc, void* stream) {
+    CMGAN_REQUIRE(dframes && x && dx, "cmgan_pad_reflect_bwd: null pointer");
+    CMGAN_REQUIRE(B >= 0 && L > NFFT / 2 && T == L / HOP + 1, "cmgan_pad_reflect_bwd: need L > 200 and T = L / 100 + 1 (L=%d T=%d)", L, T);
+    CMGAN_REQUIRE(ldx >= L && lddx >= L, "cmgan_pad_reflect_bwd: row strides must be >= L (L=%d ldx=%lld lddx=%lld)", L, ldx, lddx);
+    if (B == 0) return 0;
+    dim3 grid(cdiv(L, 256), B);
+    pad_reflect_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dframes, T, x, ldx, L, c, dx, lddx, dc);
+    return cmgan_check_launch("pad_reflect_bwd_kernel");
+}
+
+// gradient of cmgan_ola with c_div: dframes (B*T, 400) from dy / c_div, and dc[b] += -sum_n dy[b, n] y[b, n] / c_div[b] (y the forward output;
+// dc may be null; the caller zeroes it)
+CMGAN_API int cmgan_ola_div_bwd(const float* dy, long long lddy, int B, int T, const float* inv_env, const float* c_div, const float* y,
+                                long long ldy, float* dframes, float* dc, void* stream) {
+    CMGAN_REQUIRE(dy && inv_env && c_div && y && dframes, "cmgan_ola_div_bwd: null pointer");
+    CMGAN_REQUIRE(B >= 0 && T >= 2 && lddy >= (long long)HOP * (T - 1) && ldy >= (long long)HOP * (T - 1),
+                  "cmgan_ola_div_bwd: need T >= 2 and row strides >= 100 (T - 1) (T=%d lddy=%lld ldy=%lld)", T, lddy, ldy);
+    if (B == 0) return 0;
+    dim3 grid(cdiv((long)T * NFFT, 256), B);
+    ola_div_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dy, lddy, T, inv_env, c_div, y, ldy, dframes, dc);
+    return cmgan_check_launch("ola_div_bwd_kernel");
 }

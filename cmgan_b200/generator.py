@@ -153,10 +153,14 @@ class _TSCNetFn(torch.autograd.Function):
         if S is None:
             raise RuntimeError("TSCNet backward called but the forward pass did not record state")
         P = module._tensor_dict()
-        G, ret = module._grad_targets()
-        tscnet_bwd(S, dfr, dfi, P, G)
+        need_dx, need_w = ctx.needs_input_grad[0], any(ctx.needs_input_grad[4:])
+        if need_w:
+            G, ret = module._grad_targets()
+        else:       # frozen weights: no weight-gradient GEMM runs; the atomics fused into the data-gradient kernels go to scratch
+            G, ret = module._grad_scratch(), tuple(None for _ in module._param_keys)
+        dx = tscnet_bwd(S, dfr, dfi, P, G, need_dx=need_dx, need_wgrad=need_w)
         ctx.saved = None
-        return (None, None, None, None, *ret)
+        return (dx, None, None, None, *ret)
 
 
 class TSCNet(nn.Module):
@@ -216,6 +220,19 @@ class TSCNet(nn.Module):
         named = dict(self.named_parameters())
         G = {k: torch.zeros_like(named[k]) for k in self._param_keys}
         return G, tuple(G[k] if named[k].requires_grad else None for k in self._param_keys)
+
+    def _grad_scratch(self) -> Dict[str, torch.Tensor]:
+        """name -> a view of one uninitialised buffer laid out as enable_flat_grads() lays out its flat buffer (so the backward takes the
+        same GEMM forms): what the parameter-gradient atomics fused into the data-gradient kernels write when no parameter needs a gradient
+        (never read)"""
+        named = dict(self.named_parameters())
+        sizes = [((named[k].numel() + 3) // 4) * 4 for k in self._param_keys]
+        flat = torch.empty(sum(sizes), device=named[self._param_keys[0]].device)
+        G, off = {}, 0
+        for k, n in zip(self._param_keys, sizes):
+            G[k] = flat[off:off + named[k].numel()].view_as(named[k])
+            off += n
+        return G
 
     def forward(self, x: torch.Tensor, frames=None):
         """``frames`` (optional, inference only): a (B,) int sequence or tensor -- a ragged batch in which utterance b occupies frames

@@ -139,10 +139,22 @@ def tscnet_fwd(x, P, training: bool, seed: int, save: Optional[dict], frames: Op
     return fr, fi
 
 
-def tscnet_bwd(S: dict, dfr, dfi, P, G: Dict[str, torch.Tensor], after_tscb=None):
+def tscnet_bwd(S: dict, dfr, dfi, P, G: Dict[str, torch.Tensor], after_tscb=None, need_dx: bool = False, need_wgrad: bool = True):
     """Backward of tscnet_fwd.  dfr / dfi: gradients wrt final_real / final_imag ((B,1,T,F), any strides, or None).
     Parameter gradients are accumulated (+=) into the tensors of G.  ``after_tscb`` (optional callable) runs once the decoders'
-    and the TSCB stack's gradients are complete (the trainer starts their all-reduce there, under the encoder's backward)."""
+    and the TSCB stack's gradients are complete (the trainer starts their all-reduce there, under the encoder's backward).
+    ``need_dx``: also form the gradient wrt the input x and return it ((B, 2, T, F) contiguous; None otherwise).
+    ``need_wgrad=False`` (frozen weights): no weight-gradient GEMM and no head-convolution weight gradient runs; the parameter-gradient
+    atomics fused into the other backward kernels still write into G, which may then be scratch."""
+    prev = ops.WGRAD_ON
+    ops.WGRAD_ON = prev and need_wgrad
+    try:
+        return _tscnet_bwd(S, dfr, dfi, P, G, after_tscb, need_dx, need_wgrad)
+    finally:
+        ops.WGRAD_ON = prev
+
+
+def _tscnet_bwd(S, dfr, dfi, P, G, after_tscb, need_dx, need_wgrad):
     x = S["x"]
     dev = x.device
     B, T, F, F2 = S["B"], S["T"], S["F"], S["F2"]
@@ -215,5 +227,13 @@ def tscnet_bwd(S: dict, dfr, dfi, P, G: Dict[str, torch.Tensor], after_tscb=None
     draw1 = _empty(M, C, dev=dev)
     _norm_bwd(S["raw0"], C, (dcatE, 4 * C), CAT, B, T * F, C, 1, True, S["tab0"], 0, P[pe + ".conv_1.2.weight"], draw1, C,
               G[pe + ".conv_1.1.weight"], G[pe + ".conv_1.1.bias"], G[pe + ".conv_1.2.weight"], sums)
-    call("cmgan_head_conv_wgrad", x, xs[0], xs[1], xs[2], xs[3], B, T, F, draw1, C, G[pe + ".conv_1.0.weight"], G[pe + ".conv_1.0.bias"])
+    if need_wgrad:
+        call("cmgan_head_conv_wgrad", x, xs[0], xs[1], xs[2], xs[3], B, T, F, draw1, C, G[pe + ".conv_1.0.weight"], G[pe + ".conv_1.0.bias"])
+    dx = None
+    if need_dx:         # final = mask x + cplx and the head reads [|x|, re, im]: one pass over draw1 and the recomputed mask
+        dx = _empty(B, 2, T, F, dev=dev)
+        call("cmgan_tscnet_input_grad", S["m1"], tabM.scale, tabM.shift, P[pm + ".prelu.weight"], P[pm + ".final_conv.weight"],
+             P[pm + ".final_conv.bias"], P[pm + ".prelu_out.weight"], x, xs[0], xs[1], xs[2], xs[3], dfr, dfi, gs[0], gs[2], gs[3], draw1, C,
+             P[pe + ".conv_1.0.weight"], B, T, F, dx)
     ops.join_wgrad()        # weight-gradient GEMMs launched on the side stream (ops.WGRAD_STREAM) are complete from here on
+    return dx

@@ -27,6 +27,7 @@ _WGRAD_KEEP = []      # operands of in-flight side-stream launches (kept allocat
 ATTN_BWD_WS = os.environ.get("CMGAN_ATTN_BWD_WS", "0") != "0"
 PACK_CACHE = None   # optional PackCache: re-tiled tensor-core weight operands kept across calls (owner refreshes them after every weight update)
 PROBE = None     # list collecting (entry point, M, N, K, start event, end event) when bench.py instruments a step
+WGRAD_ON = True  # False while a backward runs with frozen weights (network.tscnet_bwd): every ``gemm(wgrad=True)`` is skipped
 
 PRO_NONE, PRO_LN, PRO_SWISH_DROP, PRO_BN_SWISH, PRO_DROP, PRO_IN_PRELU = range(6)
 EPI_NONE, EPI_DROP_RES, EPI_DSWISH_DROP, EPI_DBNSWISH, EPI_ACC, EPI_SWISH_DUAL = range(6)
@@ -161,7 +162,9 @@ def gemm(*, A: Ptr, lda: int, W: Ptr, sb_k: int, sb_n: int, C: Ptr, ldc: int, M:
          wgrad: bool = False, D: Ptr = None, ldd: int = 0, prod: int = 0, dbias: Ptr = None, precision: Optional[int] = None,
          C2: Ptr = None, ldc2: int = 0) -> None:
     """One dense contraction (see csrc/gemm_args.h).  ``conv`` = dict(OH, OW, IH, IW, mul_y, mul_x, div_y, div_x);
-    ``taps`` = [(dy, dx), ...].  With ``wgrad`` the call accumulates dW (laid out like W) into ``C``."""
+    ``taps`` = [(dy, dx), ...].  With ``wgrad`` the call accumulates dW (laid out like W) into ``C`` (nothing runs while ``WGRAD_ON`` is off)."""
+    if wgrad and not WGRAD_ON:
+        return
     a = GemmArgs()
     a.A, a.lda = ptr(A), lda
     a.B, a.sb_tap, a.sb_k, a.sb_n = ptr(W), sb_tap, sb_k, sb_n

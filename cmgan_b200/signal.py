@@ -50,30 +50,92 @@ def _inv_envelope_tail(dev) -> torch.Tensor:
     return _table(("env_tail", dev), (HOP,), lambda t: call("cmgan_stft_tables", None, None, 0, None, t))
 
 
-def rms_scale(wav: torch.Tensor) -> torch.Tensor:
-    """c[b] = sqrt(L / sum x^2)  (ref: train.py:75, evaluation.py:21)"""
-    assert wav.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
+def _wants_grad(*ts) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
+def _rms_scale(wav: torch.Tensor) -> torch.Tensor:
     c = torch.empty(wav.shape[0], device=wav.device)
     call("cmgan_rms_scale", wav, wav.stride(0), wav.shape[0], wav.shape[1], c)
     return c
 
 
-def stft_compress(wav: torch.Tensor, scale: torch.Tensor = None) -> torch.Tensor:
-    """(B, L) waveform (optionally scaled per utterance by ``scale``) -> power-compressed spectrogram with the shape
-    the reference's ``power_compress(torch.stft(...))`` has, (B, 2, F, T), as a permuted view of (B, 2, T, F) memory
-    (so that ``.permute(0, 1, 3, 2)`` -- train.py:95 -- yields a contiguous tensor)."""
+class _RMSScale(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, wav):
+        c = _rms_scale(wav)
+        ctx.save_for_backward(wav, c)
+        return c
+
+    @staticmethod
+    def backward(ctx, dc):
+        wav, c = ctx.saved_tensors
+        B, L = wav.shape
+        dx = torch.empty(B, L, device=wav.device)
+        call("cmgan_rms_scale_bwd", wav, wav.stride(0), B, L, c, dc.contiguous(), dx, dx.stride(0), 0)
+        return dx
+
+
+def rms_scale(wav: torch.Tensor) -> torch.Tensor:
+    """c[b] = sqrt(L / sum x^2)  (ref: train.py:75, evaluation.py:21); differentiable when ``wav`` requires grad"""
     assert wav.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
+    if _wants_grad(wav):
+        return _RMSScale.apply(wav)
+    return _rms_scale(wav)
+
+
+def _stft_compress(wav: torch.Tensor, scale: torch.Tensor = None, keep: list = None) -> torch.Tensor:
     dev = wav.device
     B, L = wav.shape
     T = L // HOP + 1
     Lp = ((L + N_FFT + HOP - 1) // HOP) * HOP
     xp = torch.empty(B, Lp, device=dev)
     call("cmgan_pad_reflect", wav, wav.stride(0), B, L, scale, xp, Lp)
-    return _stft_padded(xp, B, T).permute(0, 1, 3, 2)
+    return _stft_padded(xp, B, T, keep)
 
 
-def _stft_padded(xp: torch.Tensor, B: int, T: int) -> torch.Tensor:
-    """(B, Lp) centre-padded waveforms -> power-compressed spectrogram (B, 2, T, F), contiguous; frame t reads xp[:, 100 t : 100 t + 400]"""
+class _STFTCompress(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, wav, scale):
+        keep = []
+        X = _stft_compress(wav, scale, keep)
+        ctx.save_for_backward(wav, scale, keep[0])
+        return X
+
+    @staticmethod
+    def backward(ctx, g):
+        """g (B, 2, T, F), any strides -> the power-law gradient at the DFT output, the DFT transpose (fp32 FFMA), the adjoint of the framing,
+        reflect padding and scaling: d wav = scale * g_x and d scale = sum g_x wav"""
+        wav, scale, S = ctx.saved_tensors
+        dev = wav.device
+        B, L = wav.shape
+        T = L // HOP + 1
+        dS = torch.empty(B * T, 2 * NF, device=dev)
+        gs = g.stride()
+        call("cmgan_power_law_bwd", S, (S, NF), T * 2 * NF, 2 * NF, 1, g[:, 0], g[:, 1], gs[0], gs[2], gs[3], dS, (dS, NF), T * 2 * NF, 2 * NF, 1,
+             B, T, NF, -0.7)
+        dframes = torch.empty(B * T, N_FFT, device=dev)
+        gemm(A=dS, lda=2 * NF, W=_fwd_basis(dev), sb_k=1, sb_n=2 * NF, C=dframes, ldc=N_FFT, M=B * T, N=N_FFT, Cin=2 * NF, precision=0)
+        dx = torch.empty(B, L, device=dev)
+        dc = torch.zeros(B, device=dev) if scale is not None and ctx.needs_input_grad[1] else None
+        call("cmgan_pad_reflect_bwd", dframes, B, T, wav, wav.stride(0), L, scale, dx, dx.stride(0), dc)
+        return dx, dc
+
+
+def stft_compress(wav: torch.Tensor, scale: torch.Tensor = None) -> torch.Tensor:
+    """(B, L) waveform (optionally scaled per utterance by ``scale``) -> power-compressed spectrogram with the shape
+    the reference's ``power_compress(torch.stft(...))`` has, (B, 2, F, T), as a permuted view of (B, 2, T, F) memory
+    (so that ``.permute(0, 1, 3, 2)`` -- train.py:95 -- yields a contiguous tensor).  Differentiable wrt ``wav`` and ``scale`` when either
+    requires grad (the same launches, plus the DFT output kept for the backward)."""
+    assert wav.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
+    if _wants_grad(wav, scale):
+        return _STFTCompress.apply(wav, scale).permute(0, 1, 3, 2)
+    return _stft_compress(wav, scale).permute(0, 1, 3, 2)
+
+
+def _stft_padded(xp: torch.Tensor, B: int, T: int, keep: list = None) -> torch.Tensor:
+    """(B, Lp) centre-padded waveforms -> power-compressed spectrogram (B, 2, T, F), contiguous; frame t reads xp[:, 100 t : 100 t + 400].
+    ``keep`` (optional list) receives the DFT output S (B*T, 402) = [re | im]."""
     dev = xp.device
     Lp = xp.shape[1]
     S = torch.empty(B * T, 2 * NF, device=dev)
@@ -81,6 +143,8 @@ def _stft_padded(xp: torch.Tensor, B: int, T: int) -> torch.Tensor:
          conv=dict(OH=1, OW=T, IH=1, IW=Lp // HOP), precision=0)      # the DFTs stay exact fp32
     X = torch.empty(B, 2, T, NF, device=dev)
     call("cmgan_compress", S, B, T, X)
+    if keep is not None:
+        keep.append(S)
     return X
 
 
@@ -122,25 +186,65 @@ class _UncompressISTFT(torch.autograd.Function):
         if fi.stride() != fr.stride():
             fr, fi = fr.contiguous(), fi.contiguous()
         y = uncompress_istft_fwd(fr, fi, c_div)
-        ctx.save_for_backward(fr, fi)
         ctx.has_c = c_div is not None
+        if ctx.has_c:
+            ctx.save_for_backward(fr, fi, c_div, y)
+        else:
+            ctx.save_for_backward(fr, fi)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        fr, fi = ctx.saved_tensors
-        assert not ctx.has_c, "the de-normalised (evaluation) path is inference only"
-        B, _, T, F = fr.shape
-        dre = torch.empty(B, 1, T, F, device=fr.device)
-        dim = torch.empty(B, 1, T, F, device=fr.device)
-        uncompress_istft_bwd(fr, fi, dy.contiguous(), dre, dim, False)
-        return dre, dim, None
+        B = dy.shape[0]
+        dy = dy.contiguous()
+        if not ctx.has_c:
+            fr, fi = ctx.saved_tensors
+            B, _, T, F = fr.shape
+            dre = torch.empty(B, 1, T, F, device=fr.device)
+            dim = torch.empty(B, 1, T, F, device=fr.device)
+            uncompress_istft_bwd(fr, fi, dy, dre, dim, False)
+            return dre, dim, None
+        # de-normalised: y = ola(frames) / c_div -> d frames = ola_bwd(dy / c_div), d c_div = -sum dy y / c_div
+        fr, fi, c_div, y = ctx.saved_tensors
+        dev = fr.device
+        _, _, T, F = fr.shape
+        dframes = torch.empty(B * T, N_FFT, device=dev)
+        dc = torch.zeros(B, device=dev) if ctx.needs_input_grad[2] else None
+        call("cmgan_ola_div_bwd", dy, dy.stride(0), B, T, _inv_envelope(T, dev), c_div, y, y.stride(0), dframes, dc)
+        dU = torch.empty(B * T, 2 * NF, device=dev)
+        gemm(A=dframes, lda=N_FFT, W=_inv_basis(dev), sb_k=1, sb_n=N_FFT, C=dU, ldc=2 * NF, M=B * T, N=2 * NF, Cin=N_FFT, precision=0)
+        dre = torch.empty(B, 1, T, F, device=dev)
+        dim = torch.empty(B, 1, T, F, device=dev)
+        s = fr.stride()
+        call("cmgan_uncompress_bwd", fr, fi, s[0], s[2], s[3], B, T, dU, dre, dim, 0)
+        return dre, dim, dc
 
 
 def uncompress_istft(final_real: torch.Tensor, final_imag: torch.Tensor, c_div: torch.Tensor = None) -> torch.Tensor:
     """(B, 1, T, F) x 2 (TSCNet outputs, any strides) -> waveform (B, 100 (T - 1)); differentiable.
-    ``c_div``: optional per-utterance divisor (evaluation.py:51 de-normalisation)."""
+    ``c_div``: optional per-utterance divisor (evaluation.py:51 de-normalisation), contiguous (B,); differentiable too."""
     return _UncompressISTFT.apply(final_real, final_imag, c_div)
+
+
+def enhance_grad(model, noisy: torch.Tensor, cut_len: int = 16000 * 16) -> torch.Tensor:
+    """``enhance_batch`` with autograd: (B, L) clips of one length (wrap-padded length <= cut_len) -> (B, L) enhanced clips, differentiable
+    wrt ``noisy`` and the model's parameters through RMS normalisation, wrap padding, STFT, compression, TSCNet, un-compression, iSTFT and
+    de-normalisation.  The values are those of ``enhance_batch``, bit for bit: the forward runs the same kernels.  The one intended difference
+    from the reference's autograd: where a bin of the noisy spectrogram is exactly 0, the magnitude term of TSCNet's input gradient is 0
+    (the reference's sqrt gives NaN there)."""
+    assert noisy.dim() == 2
+    noisy = noisy.contiguous()
+    B, length = noisy.shape
+    padded_len = int(math.ceil(length / 100)) * 100
+    if padded_len > cut_len:
+        raise ValueError(f"enhance_grad: clips of {length} samples (padded {padded_len}) exceed cut_len = {cut_len}; the folding path has "
+                         "no gradient")
+    c = rms_scale(noisy)
+    if padded_len != length:
+        noisy = torch.cat([noisy, noisy[:, :padded_len - length]], dim=-1)
+    spec = stft_compress(noisy, c).permute(0, 1, 3, 2)
+    fr, fi = model(spec)
+    return uncompress_istft(fr, fi, c)[:, :length]
 
 
 @torch.no_grad()

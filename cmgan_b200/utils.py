@@ -10,17 +10,41 @@ _P_COMPRESS = 0.3 - 1.0            # |X|^0.3 e^{j angle X} = X |X|^-0.7
 _P_UNCOMPRESS = 1.0 / 0.3 - 1.0    # |Y|^(1/0.3) e^{j angle Y} = Y |Y|^(7/3)
 
 
-def power_compress(x: torch.Tensor) -> torch.Tensor:
-    """x: (B, F, T, 2) real view of a complex STFT -> (B, 2, F, T)   (ref: utils.py:20-29)"""
-    if not x.is_cuda:
-        raise RuntimeError("cmgan_b200.power_compress runs on CUDA only")
+def _power_compress(x: torch.Tensor) -> torch.Tensor:
     B, F, T, two = x.shape
-    assert two == 2
     out = torch.empty(B, 2, F, T, device=x.device, dtype=torch.float32)
     re, im = x[..., 0], x[..., 1]
     s, so = re.stride(), out[:, 0].stride()
     call("cmgan_power_law", re, im, s[0], s[1], s[2], out[:, 0], out[:, 1], so[0], so[1], so[2], B, F, T, _P_COMPRESS)
     return out
+
+
+class _Compress(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return _power_compress(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        B, F, T, _ = x.shape
+        dx = torch.empty(B, F, T, 2, device=x.device)
+        s, gs = x[..., 0].stride(), g[:, 0].stride()
+        call("cmgan_power_law_bwd", x[..., 0], x[..., 1], s[0], s[1], s[2], g[:, 0], g[:, 1], gs[0], gs[1], gs[2], dx[..., 0], dx[..., 1],
+             F * T * 2, T * 2, 2, B, F, T, _P_COMPRESS)
+        return dx
+
+
+def power_compress(x: torch.Tensor) -> torch.Tensor:
+    """x: (B, F, T, 2) real view of a complex STFT -> (B, 2, F, T)   (ref: utils.py:20-29); differentiable when x requires grad
+    (the gradient is 0 where X = 0)"""
+    if not x.is_cuda:
+        raise RuntimeError("cmgan_b200.power_compress runs on CUDA only")
+    assert x.shape[-1] == 2
+    if torch.is_grad_enabled() and x.requires_grad:
+        return _Compress.apply(x)
+    return _power_compress(x)
 
 
 class _Uncompress(torch.autograd.Function):

@@ -95,6 +95,17 @@ int cmgan_rowdot_bwd(const float* in, int B, int T, int Fout, int nout, const fl
 int cmgan_recombine(const float* m1, const float* in_scale, const float* in_shift, const float* a1, const float* fcw, const float* fcb, const float* slope_f, const float* x, long long sb, long long sc, long long st, long long sf, const float* cplx, int B, int T, int F, float* fr, float* fi, void* stream);
 int cmgan_recombine_bwd(const float* m1, const float* in_scale, const float* in_shift, const float* a1, const float* fcw, const float* fcb, const float* slope_f, const float* x, long long sb, long long sc, long long st, long long sf, const float* dfr, const float* dfi, long long gb, long long gt, long long gf, int B, int T, int F, float* dcplx, float* dz, float* dslope_f, float* dfcw, float* dfcb, void* stream);
 
+/* ---- input gradients: TSCNet and the signal front end differentiated wrt their inputs (dc / dc_div are accumulated: zero them first).
+ * cmgan_tscnet_input_grad: dx (B, 2, T, F) contiguous from dfr / dfi, the mask tail (as cmgan_recombine_bwd) and draw (M, ldd), the gradient of
+ *   the raw head-convolution output (16-byte aligned, ldd % 4 == 0); w = the head weight (64, 3).  Where |x| = 0 the magnitude term is 0.
+ * cmgan_rms_scale_bwd: dx (+)= -dc c^3 x / L.  cmgan_pad_reflect_bwd: dframes (B*T, 400), T = L / 100 + 1, -> dx = c g and dc += sum g x, the
+ *   adjoint of cmgan_pad_reflect and the DFT's framing (c, dc may be null).  cmgan_ola_div_bwd: the gradient of cmgan_ola with c_div (y = its
+ *   output; dc may be null). */
+int cmgan_tscnet_input_grad(const float* m1, const float* in_scale, const float* in_shift, const float* a1, const float* fcw, const float* fcb, const float* slope_f, const float* x, long long sb, long long sc, long long st, long long sf, const float* dfr, const float* dfi, long long gb, long long gt, long long gf, const float* draw, long long ldd, const float* w, int B, int T, int F, float* dx, void* stream);
+int cmgan_rms_scale_bwd(const float* x, long long ldx, int B, int L, const float* c, const float* dc, float* dx, long long lddx, int accumulate, void* stream);
+int cmgan_pad_reflect_bwd(const float* dframes, int B, int T, const float* x, long long ldx, int L, const float* c, float* dx, long long lddx, float* dc, void* stream);
+int cmgan_ola_div_bwd(const float* dy, long long lddy, int B, int T, const float* inv_env, const float* c_div, const float* y, long long ldy, float* dframes, float* dc, void* stream);
+
 /* ---- discriminator-only pieces (discriminator.py:29-64, utils.py:42-50) and dropout-mask export */
 int cmgan_dropout_mask(float* out, long long n, unsigned long long seed, unsigned int thr, void* stream);
 int cmgan_stack2(const float* x, long long xb, long long xh, long long xw, const float* y, long long yb, long long yh, long long yw, int B, int H, int W, float* out, void* stream);
