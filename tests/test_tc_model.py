@@ -1,12 +1,13 @@
 """The exact model the tf32 tensor-core tests compare against (tests/tf32_model.py), checked on the CPU: the two operand-rounding
-emulators against an independent float64 formula, and the implicit-convolution builder against a literal row gather."""
+emulators against an independent float64 formula, the implicit-convolution builder against a literal row gather, and its
+weight-gradient transpose against a literal row gather and autograd's conv2d_weight."""
 import math
 
 import numpy as np
 import pytest
 import torch
 
-from tf32_model import conv_rows, conv_rows_gather, tf32_exact, tf32_rna, tf32_rz, weight_taps
+from tf32_model import conv_rows, conv_rows_gather, tf32_exact, tf32_rna, tf32_rz, weight_taps, wgrad_taps, wgrad_taps_gather
 
 
 def _ulp_tf32(a: float) -> float:
@@ -103,6 +104,65 @@ def test_conv_rows_matches_row_gather(form):
     want = conv_rows_gather(A, Wt, M, taps, conv)
     assert want.abs().max() > 0
     torch.testing.assert_close(got, want, rtol=1e-12, atol=1e-12)
+
+
+def _wgrad_form(form):
+    """(conv, taps) of every gather form the weight-gradient GEMM runs: same-size (causal dilated dense block, dilation > T, sub-pixel),
+    strided along F (encoder conv_2), the discriminator's 4 x 4 stride-2 convolution with padding 1"""
+    if form == "same":
+        return dict(OH=4, OW=5, IH=4, IW=5), [(-1, -1), (0, 0), (1, 1), (0, -1)]
+    if form == "dense_dil2":
+        return dict(OH=5, OW=4, IH=5, IW=4), [((kh - 1) * 2, kw - 1) for kh in range(2) for kw in range(3)]
+    if form == "dense_dil8":              # T < 8: the dy = -8 taps read padding only
+        return dict(OH=3, OW=5, IH=3, IW=5), [((kh - 1) * 8, kw - 1) for kh in range(2) for kw in range(3)]
+    if form == "subpixel":
+        return dict(OH=3, OW=6, IH=3, IW=6), [(0, -1), (0, 0), (0, 1)]
+    if form == "mul_x":
+        return dict(OH=3, OW=4, IH=3, IW=7, mul_x=2), [(0, -1), (0, 0), (0, 1)]
+    return dict(OH=3, OW=4, IH=6, IW=8, mul_y=2, mul_x=2), [(kh - 1, kw - 1) for kh in range(4) for kw in range(4)]
+
+
+@pytest.mark.parametrize("form", ["same", "dense_dil2", "dense_dil8", "subpixel", "mul_x", "mul_yx"])
+def test_wgrad_taps_matches_row_gather(form):
+    g = torch.Generator().manual_seed(5)
+    conv, taps = _wgrad_form(form)
+    B, Cin, N = 2, 5, 3
+    M = B * conv["OH"] * conv["OW"]
+    A = torch.randn(B * conv["IH"] * conv["IW"], Cin, generator=g, dtype=torch.float64)
+    D = torch.randn(M, N, generator=g, dtype=torch.float64)
+    got = wgrad_taps(A, D, M, taps, conv)
+    want = wgrad_taps_gather(A, D, M, taps, conv)
+    assert got.shape == (len(taps), Cin, N) and want.abs().max() > 0
+    torch.testing.assert_close(got, want, rtol=1e-12, atol=1e-12)
+    # the transpose of conv_rows: <conv_rows(A, W), D> = <W, wgrad_taps(A, D)> for any W
+    W = torch.randn(len(taps), Cin, N, generator=g, dtype=torch.float64)
+    torch.testing.assert_close((conv_rows(A, W, M, taps, conv) * D).sum(), (W * got).sum(), rtol=1e-12, atol=1e-12)
+    if form == "dense_dil8":
+        assert got[:3].abs().max() == 0, "taps that read padding only contribute nothing"
+
+
+@pytest.mark.parametrize("dil", [1, 2, 4, 8])
+def test_wgrad_taps_matches_conv2d_weight(dil):
+    """the dense block's causal dilated 2 x 3 convolution read from a column slice of the concat buffer, against autograd's own
+    weight gradient: padding (dil, 1) on both sides, the first T output rows are the causal ones"""
+    g = torch.Generator().manual_seed(6)
+    B, T, Fw, Cin, N, c0 = 2, 9, 7, 6, 4, 3
+    cat = torch.randn(B * T * Fw, 12, generator=g, dtype=torch.float64)
+    D = torch.randn(B * T * Fw, N, generator=g, dtype=torch.float64)
+    taps = [((kh - 1) * dil, kw - 1) for kh in range(2) for kw in range(3)]
+    got = wgrad_taps(cat[:, c0:c0 + Cin], D, B * T * Fw, taps, dict(OH=T, OW=Fw, IH=T, IW=Fw))
+    x = cat[:, c0:c0 + Cin].reshape(B, T, Fw, Cin).permute(0, 3, 1, 2)
+    dy = torch.zeros(B, N, T + dil, Fw, dtype=torch.float64)
+    dy[:, :, :T] = D.view(B, T, Fw, N).permute(0, 3, 1, 2)
+    gw = torch.nn.grad.conv2d_weight(x, (N, Cin, 2, 3), dy, padding=(dil, 1), dilation=(dil, 1))      # (N, Cin, kh, kw)
+    torch.testing.assert_close(got, gw.permute(2, 3, 1, 0).reshape(6, Cin, N), rtol=1e-12, atol=1e-12)
+
+
+def test_wgrad_taps_dense_rows():
+    g = torch.Generator().manual_seed(7)
+    A, D = torch.randn(9, 40, generator=g, dtype=torch.float64), torch.randn(9, 3, generator=g, dtype=torch.float64)
+    got = wgrad_taps(A[:, 8:12], D, 7)            # a column slice of A, the first M rows
+    torch.testing.assert_close(got, sum(torch.outer(A[m, 8:12], D[m]) for m in range(7)).unsqueeze(0), rtol=1e-14, atol=1e-14)
 
 
 def test_conv_rows_dense():
