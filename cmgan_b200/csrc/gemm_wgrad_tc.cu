@@ -13,6 +13,7 @@
 // columns on the Q side (P = A), or n on the M side and all Cin columns on the Q side (P = D, Cin <= 256).  At the end each CTA adds its
 // tile into dW (and, for one tile per tap-0 column range, its column sums into dbias) with atomics: the parameter-gradient buffer is
 // zeroed once per step.  The grid is as many CTAs as are resident at once (one wave).
+// The dense blocks' dilated 2 x 3 convolutions take a second plan that covers all six taps in one tile (gemm_wgrad_taps_kernel below).
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
 #include "gemm_device.cuh"
@@ -237,6 +238,185 @@ __global__ void __launch_bounds__(NT, NB <= 3 ? 2 : 1) gemm_wgrad_tc_kernel(cons
     }
 }
 
+// ---- the dense block's causal dilated 2 x 3 convolution: all six taps in one tile -------------------------------------------------
+// Taps (dy, dx) = ((kh - 1) dil, kw - 1), tap = 3 kh + kw, stride 1, same size.  Indexed by the input row r instead of the output row m,
+//     dW(tap, k, n) = sum_r A[r, k] D[r - dy IW - dx, n]      (only where row r - dy IW - dx reads r through the tap)
+// so one K-major image of a stage's 32 A rows serves every tap, and each tap reads D shifted by its offset.  The shift is along the
+// wgmma K dimension, which a shared-memory descriptor cannot offset by single rows, so D^T goes to the M side from registers: each
+// thread loads its fragment straight from a row-major D window at the tap's row, masks it and rounds it.  Warpgroup h takes the taps
+// kh = h (three m64n64 accumulators, 96 registers): kh = 1 reads the window of the stage's own rows, kh = 0 one dil IW rows further,
+// each with a one-row halo for dx = +-1.  A CTA owns 64 A columns and a range of A rows; dbias comes from tap (0, 0) of column tile 0.
+constexpr int TQ = 64;               // A columns per CTA
+constexpr int DWP = 72;              // D window row pitch (floats): 72 = 8 mod 32 banks, so the fragment loads are conflict-free
+constexpr int DWR = RS + 2;          // D window rows: the stage's 32 and one each side
+constexpr uint32_t TAPS_A = RS * TQ * 4, TAPS_WIN = DWR * DWP * 4, TAPS_MASK = 2 * TAPS_WIN + TAPS_A;
+constexpr uint32_t TAPS_RAW = TAPS_MASK + RS * 4, TAPS_IMG = TQ * 128;
+
+struct TapsPlan {
+    int ring;              // slabs in the cp.async ring
+    int mch;               // A rows per CTA, a multiple of RS
+};
+
+// bit t: A row r feeds tap t, i.e. row m = r - dy IW - dx lies in the same image row (x - dx inside [0, IW)), the same utterance and < M
+__device__ __forceinline__ uint32_t taps_mask(const CmganGemmArgs& g, int r, int dil) {
+    const int x = r % g.IW, y = (r / g.IW) % g.IH;
+    uint32_t mk = 0;
+#pragma unroll
+    for (int t = 0; t < 6; ++t) {
+        const int kh = t / 3, dx = t % 3 - 1;
+        const long m = (long)r + (kh ? 0 : (long)dil * g.IW) - dx;
+        if (x - dx >= 0 && x - dx < g.IW && (kh || y + dil < g.IH) && m < g.M) mk |= 1u << t;
+    }
+    return mk;
+}
+
+__global__ void __launch_bounds__(NT, 1) gemm_wgrad_taps_kernel(const __grid_constant__ CmganGemmArgs g, const TapsPlan p) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* const bptr = smem_raw + (base - smem_u32(smem_raw));
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int acol0 = blockIdx.x * TQ, dil = -g.dy[0];
+    const long shift = (long)dil * g.IW;
+    const long rbeg = (long)blockIdx.y * p.mch;
+    const long rend = rbeg + p.mch < g.M ? rbeg + p.mch : g.M;
+    const int nst = (int)((rend - rbeg + RS - 1) / RS);
+    if (nst <= 0) return;
+    const bool do_bias = g.dbias != nullptr && blockIdx.x == 0;
+    uint8_t* const img0 = bptr;
+    uint8_t* const ring = bptr + 2 * TAPS_IMG;
+
+    // stage s -> slab: thread t copies A row t / 8 (16-byte chunks t % 8, t % 8 + 8), the last warp writes the rows' tap masks; then
+    // the 2 x 34 rows of the two D windows (window kh starts at D row r0 - 1 + (1 - kh) dil IW), 16 chunks each, rows outside [0, M)
+    // left unwritten
+    auto issue = [&](int s, int slot) {
+        uint8_t* const sl = ring + slot * TAPS_RAW;
+        const long r0 = rbeg + (long)s * RS;
+        const int row = tid >> 3, c8 = tid & 7;
+        const long r = r0 + row;
+        if (r < rend) {
+            const float* src = g.A + g.tap_off[0] + r * g.lda + acol0;
+            cp_async16(smem_u32(sl + raw_off(row, c8, TQ)), src + 4 * c8, 16);
+            cp_async16(smem_u32(sl + raw_off(row, c8 + 8, TQ)), src + 4 * c8 + 32, 16);
+        }
+        if (warp == NT / 32 - 1) {    // one warp decodes the stage's 32 rows: a divergent branch in every warp would cost each of them
+            const long rl = r0 + lane;
+            reinterpret_cast<uint32_t*>(sl + TAPS_MASK)[lane] = rl < rend ? taps_mask(g, (int)rl, dil) : 0u;
+        }
+        for (int i = tid; i < 2 * DWR * 16; i += NT) {
+            const int kh = i / (DWR * 16), j = i % (DWR * 16), wr = j >> 4, c = j & 15;
+            const long m = r0 - 1 + wr + (kh ? 0 : shift);
+            if (m >= 0 && m < g.M) cp_async16(smem_u32(sl + TAPS_A + kh * TAPS_WIN + (wr * DWP + 4 * c) * 4), g.D + m * g.ldd + 4 * c, 16);
+        }
+    };
+
+    // A rows -> K-major SWIZZLE_128B image: thread t < 128 transposes A lines 4 lb .. 4 lb + 3 x rows 4 q .. 4 q + 3 (lb = t / 8, q = t % 8)
+    auto transform = [&](int s, int slot, uint8_t* img) {
+        if (tid >= 2 * TQ) return;
+        const uint8_t* const sl = ring + slot * TAPS_RAW;
+        const long mb = rbeg + (long)s * RS;
+        const int lb = tid >> 3, q = tid & 7;
+        float4 v[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)         // rows past the CTA's range are zero: another CTA owns them
+            v[i] = mb + 4 * q + i < rend ? round4(*reinterpret_cast<const float4*>(sl + raw_off(4 * q + i, lb, TQ)))
+                                         : make_float4(0.f, 0.f, 0.f, 0.f);
+        const int L = 4 * lb;
+        *reinterpret_cast<float4*>(img + (L + 0) * 128 + (((q ^ (L + 0)) & 7) << 4)) = make_float4(v[0].x, v[1].x, v[2].x, v[3].x);
+        *reinterpret_cast<float4*>(img + (L + 1) * 128 + (((q ^ (L + 1)) & 7) << 4)) = make_float4(v[0].y, v[1].y, v[2].y, v[3].y);
+        *reinterpret_cast<float4*>(img + (L + 2) * 128 + (((q ^ (L + 2)) & 7) << 4)) = make_float4(v[0].z, v[1].z, v[2].z, v[3].z);
+        *reinterpret_cast<float4*>(img + (L + 3) * 128 + (((q ^ (L + 3)) & 7) << 4)) = make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
+    };
+
+    // fragment of this thread: D columns n0, n0 + 8 (the M side), A rows 8 j + 4 h + tq of the stage (the K side)
+    const int n0 = 16 * (warp & 3) + (lane >> 2), tq = lane & 3;
+    float acc[3][4][8];                    // written first by the MMAs of stage 0 (nst >= 1)
+    // dbias: columns n0, n0 + 8 (warpgroup 1, tap (0, 0)), compensated sums: a thread adds up to a quarter of its CTA's rows
+    float cs0 = 0.f, cs1 = 0.f, cc0 = 0.f, cc1 = 0.f;
+    auto kahan = [](float& sum, float& c, float v) {
+        const float y = v - c, t = sum + y;
+        c = (t - sum) - y;
+        sum = t;
+    };
+
+    for (int s = 0; s < p.ring - 1; ++s) {
+        if (s < nst) issue(s, s);
+        cp_async_commit();
+    }
+    for (int s = 0; s < nst; ++s) {
+        cp_async_wait_n(p.ring - 2);
+        __syncthreads();              // stage s visible to all; slab s - 1 and image s - 2 are no longer read
+        if (s + p.ring - 1 < nst) issue(s + p.ring - 1, (s + p.ring - 1) % p.ring);
+        cp_async_commit();
+        uint8_t* const img = img0 + (s & 1) * TAPS_IMG;
+        transform(s, s % p.ring, img);
+        fence_proxy_async();
+        __syncthreads();
+        wgmma_wait<0>();              // the MMAs of stage s - 1 are done: their fragment registers may be overwritten
+        const uint8_t* const sl = ring + (s % p.ring) * TAPS_RAW;
+        const float* const win = reinterpret_cast<const float*>(sl + TAPS_A + wg * TAPS_WIN) + n0;
+        const uint32_t* const mask = reinterpret_cast<const uint32_t*>(sl + TAPS_MASK);
+        uint32_t fr[4][3][4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int kk = 8 * j + 4 * h + tq;
+                const uint32_t mk = mask[kk] >> (3 * wg);
+#pragma unroll
+                for (int kw = 0; kw < 3; ++kw) {
+                    const float* const src = win + (kk + 2 - kw) * DWP;      // D row r - dx, window row r - r0 + 1 - dx
+                    const bool ok = (mk >> kw) & 1u;
+                    const float v0 = ok ? src[0] : 0.f, v1 = ok ? src[8] : 0.f;
+                    fr[j][kw][2 * h] = __float_as_uint(to_tf32(v0));
+                    fr[j][kw][2 * h + 1] = __float_as_uint(to_tf32(v1));
+                    if (kw == 1 && wg == 1 && do_bias) { kahan(cs0, cc0, v0); kahan(cs1, cc1, v1); }
+                }
+            }
+        }
+        const uint64_t bdesc = gmma_desc_sw128(smem_u32(img));
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int kw = 0; kw < 3; ++kw) wgmma_m64n64k8_tf32_rs(acc[kw], fr[j][kw], bdesc + (uint64_t)(2 * j), (s == 0 && j == 0) ? 0u : 1u);
+        wgmma_commit();
+    }
+    wgmma_wait<0>();
+
+    // accumulator fragment: M row n0 + 8 ((e >> 1) & 1), N column 16 b + 8 (e >> 2) + 2 tq + (e & 1)
+    const int kh = wg;
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) {
+        float* const dst = g.C + (long)(3 * kh + kw) * g.sb_tap;
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int n = n0 + 8 * ((e >> 1) & 1), k = acol0 + 16 * b + 8 * (e >> 2) + 2 * tq + (e & 1);
+                atomicAdd(dst + (long)k * g.sb_k + (long)n * g.sb_n, acc[kw][b][e]);
+            }
+    }
+    if (do_bias && wg == 1) {
+        cs0 += __shfl_xor_sync(0xffffffffu, cs0, 1);
+        cs0 += __shfl_xor_sync(0xffffffffu, cs0, 2);
+        cs1 += __shfl_xor_sync(0xffffffffu, cs1, 1);
+        cs1 += __shfl_xor_sync(0xffffffffu, cs1, 2);
+        if (tq == 0) { atomicAdd(g.dbias + n0, cs0); atomicAdd(g.dbias + n0 + 8, cs1); }
+    }
+}
+
+// the dense block's convolution, which the taps plan covers: stride 1, same size, taps ((kh - 1) dil, kw - 1) in kh-major order, one A
+// pointer for every tap, no prologue and no scale on D, N = 64 and whole 64-column tiles of A
+bool taps_plan_fits(const CmganGemmArgs* a) {
+    if (!a->conv || a->ntaps != 6 || a->mul_y != 1 || a->mul_x != 1 || a->div_y != 1 || a->div_x != 1) return false;
+    if (a->OH != a->IH || a->OW != a->IW || a->pro != CMGAN_PRO_NONE || a->prod != 0 || a->N != 64 || a->Cin % TQ) return false;
+    const int dil = -a->dy[0];
+    if (dil < 1) return false;
+    for (int t = 0; t < 6; ++t)
+        if (a->dy[t] != (t / 3 - 1) * dil || a->dx[t] != t % 3 - 1 || a->tap_off[t] != a->tap_off[0]) return false;
+    return true;
+}
+
 int wgrad_tc_supported(const CmganGemmArgs* a) {
     if (a->N % 16 || a->N < 16 || a->N > QMAX) return 0;
     if (a->Cin % 4 || a->lda % 4 || ((uintptr_t)a->A & 15) || a->ldd % 4 || ((uintptr_t)a->D & 15)) return 0;
@@ -284,6 +464,31 @@ int launch(const CmganGemmArgs* a, Plan p, size_t smem, int smem_blk, cudaStream
     return cmgan_check_launch("gemm_wgrad_tc_kernel");
 }
 
+// one CTA per SM (the accumulators take 96 registers a thread), one wave: the column tiles x row chunks fill the SMs once
+int launch_taps(const CmganGemmArgs* a, int smem_blk, cudaStream_t st) {
+    TapsPlan p{};
+    const long ring = (smem_blk - 1024 - 2L * TAPS_IMG) / TAPS_RAW;
+    if (ring < 3) { cmgan_set_error("gemm_wgrad_taps: the ring does not fit in shared memory"); return -1; }
+    p.ring = ring > MAX_RING ? MAX_RING : (int)ring;
+    const size_t smem = 1024 + 2 * (size_t)TAPS_IMG + (size_t)p.ring * TAPS_RAW;
+    static bool attr_set = false;
+    if (!attr_set) {
+        cudaError_t e = cudaFuncSetAttribute(gemm_wgrad_taps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_blk);
+        if (e != cudaSuccess) { cmgan_set_error("gemm_wgrad_taps: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return -1; }
+        attr_set = true;
+    }
+    const long tiles = a->Cin / TQ;
+    long chunks = (long)cmgan_num_sms() / tiles;
+    if (chunks < 1) chunks = 1;
+    const long max_chunks = (a->M + RS - 1) / RS;
+    if (chunks > max_chunks) chunks = max_chunks;
+    const long mch = (a->M + chunks - 1) / chunks;
+    p.mch = (int)(((mch + RS - 1) / RS) * RS);
+    const dim3 grid((unsigned)tiles, (unsigned)((a->M + p.mch - 1) / p.mch));
+    gemm_wgrad_taps_kernel<<<grid, NT, smem, st>>>(*a, p);
+    return cmgan_check_launch("gemm_wgrad_taps_kernel");
+}
+
 }  // namespace
 
 // tf32 tensor-core path of cmgan_gemm_wgrad (same contract, bias gradient included).  Returns 1 if the shape is not covered (the caller
@@ -293,6 +498,7 @@ int cmgan_gemm_wgrad_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
     if (a->M <= 0) return 0;
     int smem_sm, smem_blk;
     if (smem_limits(&smem_sm, &smem_blk)) return -1;
+    if (taps_plan_fits(a)) return launch_taps(a, smem_blk, st);
     Plan p{};
     // orientation: the one that reads fewer bytes of A and D in total (every tile reads all rows of its columns)
     const long cost_x = (long)cdiv(a->Cin, PT) * (PT + a->N), cost_y = (long)cdiv(a->N, PT) * (a->Cin + PT);

@@ -100,6 +100,16 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[4][8], uint64_t a
                  : CMGAN_D8(0), CMGAN_D8(1), CMGAN_D8(2), CMGAN_D8(3)
                  : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// the same with A from registers: a[0..3] = tf32 elements (row 16 w + l / 4, column l % 4), (row + 8, column), (row, column + 4),
+// (row + 8, column + 4) of warp w's 16 x 8 slice of A.  They must not be overwritten until a wgmma_wait covers this instruction.
+__device__ __forceinline__ void wgmma_m64n64k8_tf32_rs(float (&d)[4][8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+                 : CMGAN_D8(0), CMGAN_D8(1), CMGAN_D8(2), CMGAN_D8(3)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 #undef CMGAN_D8
 
 // one 32-float K chunk (4 instructions along K) of a 64 x (16 NB) accumulator: both operands K-major SWIZZLE_128B, the B rows 16 at a
