@@ -8,6 +8,7 @@
 // Parameters: one flat fp32 block holding every floating-point tensor of the reference's state_dict, in state_dict order, each tensor
 // starting at a multiple of 4 floats (cmgan_tscnet_param_info enumerates key / offset / element count; the int64 num_batches_tracked
 // buffers are not part of it).
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <unordered_map>
@@ -98,24 +99,74 @@ const std::unordered_map<std::string, long long>& offsets() {
     return m;
 }
 
+struct Tabs { float *scale, *shift, *mean, *rstd; int width; };
+
+// ---- what the backward reads, kept by a training forward (cmgan_tscnet_fwd_train) in the saved region of the workspace
+struct FfSaved { float *xn = nullptr, *st = nullptr, *h = nullptr, *a = nullptr; };      // fp32 feed-forward only (tf32 recomputes its hidden layer)
+struct ConfSaved {
+    const float* x;             // block input (the previous block's output)
+    float *x1, *xn2, *st2, *qkv, *ctx, *lse, *x2, *xn3, *st3, *g, *d, *dsw, *x3, *x4, *st5;
+    Tabs bn;
+    FfSaved f1, f2;
+};
+struct DenseSaved { float* raw[4]; Tabs tab[4]; };
+struct Saved {
+    float *catE, *raw0, *e2;
+    Tabs tab0, tab2;
+    DenseSaved enc;
+    ConfSaved conf[8];
+    float *cat[2], *sp[2];
+    DenseSaved dec[2];
+    float* m1;
+    Tabs tabM, tabC;
+};
+
+// counter-based dropout parameters (ops.drop_params) and per-site seeds (conformer_block._site_seed)
+constexpr double P_DROP = 0.2;          // generator.py:81-82,88-89: attention and feed-forward dropout
+unsigned drop_thr(bool on) { return on ? (unsigned)std::min(P_DROP * 4294967296.0, 4294967295.0) : 0u; }
+float drop_inv(bool on) { return on ? (float)(1.0 / (1.0 - P_DROP)) : 1.f; }
+unsigned long long site_seed(unsigned long long seed, int block_id, int site) { return seed * 1000003ull + (unsigned long long)(block_id * 16 + site + 1); }
+
+template <typename T>
+T* off(T* p, long long n) { return p ? p + n : nullptr; }
+
 // ---- one forward pass = a walk over the launch list; `dry` only sizes the workspace
 struct Run {
     const float* P;             // parameter block (null in a dry run)
-    char* ws;                   // workspace base
+    char* ws;                   // workspace base (of the scratch region when `sv` is set)
     size_t top = 0, peak = 0, cap = 0;
     bool dry;
     int precision;
     cudaStream_t st;
     const int* frames = nullptr;      // ragged batch: valid frames per utterance (device); null = every utterance fills the grid
     int rc = 0;
+    // training entries only (the inference walks leave these alone)
+    Saved* sv = nullptr;        // forward: keep what the backward reads in the saved region (below the scratch) and record where
+    char* kws = nullptr;        // saved region base
+    size_t ktop = 0;
+    bool quiet = false;         // walk for the addresses only: the backward re-derives the saved layout this way, nothing is launched
+    bool training = false;      // dropout and BatchNorm batch statistics (running statistics updated in place)
+    unsigned long long seed = 0;
+    const unsigned long long* seed_dev = nullptr;
+    float* G = nullptr;         // backward: parameter-gradient block (scratch when the weights are frozen)
+    bool wgrad = true;          // backward: run the weight-gradient GEMMs and the head weight gradient
 
+    long long find(const std::string& key) const {
+        const auto it = offsets().find(key);
+        if (it != offsets().end()) return it->second;
+        cmgan_set_error("cmgan_tscnet: unknown parameter %s", key.c_str());
+        const_cast<Run*>(this)->rc = -1;
+        return -1;
+    }
     const float* w(const std::string& key) const {
         if (dry) return nullptr;
-        const auto it = offsets().find(key);
-        if (it != offsets().end()) return P + it->second;
-        cmgan_set_error("cmgan_tscnet_fwd: unknown parameter %s", key.c_str());
-        const_cast<Run*>(this)->rc = -1;
-        return nullptr;
+        const long long o = find(key);
+        return o < 0 ? nullptr : P + o;
+    }
+    float* g(const std::string& key) const {
+        if (dry) return nullptr;
+        const long long o = find(key);
+        return o < 0 ? nullptr : G + o;
     }
     template <typename T = float>
     T* alloc(size_t n) {
@@ -126,21 +177,30 @@ struct Run {
         if (!dry && top > cap && rc == 0) { cmgan_set_error("cmgan_tscnet_fwd: workspace too small (%zu bytes needed so far, %zu given)", top, cap); rc = -1; }
         return p;
     }
+    // an activation the backward reads: in the saved region when saving, else scratch like any other buffer
+    template <typename T = float>
+    T* keep(size_t n) {
+        if (!sv) return alloc<T>(n);
+        ktop = (ktop + 255) & ~(size_t)255;
+        T* p = dry ? nullptr : reinterpret_cast<T*>(kws + ktop);
+        ktop += n * sizeof(T);
+        return p;
+    }
     void ok(int r) { if (r != 0 && rc == 0) rc = r; }
-    bool live() const { return !dry && rc == 0; }
+    bool live() const { return !dry && !quiet && rc == 0; }
 };
 
-struct Tabs { float *scale, *shift, *mean, *rstd; int width; };
 Tabs make_tabs(Run& r, int G, int width) {
     Tabs t;
-    t.scale = r.alloc((size_t)G * width); t.shift = r.alloc((size_t)G * width);
-    t.mean = r.alloc((size_t)G * width); t.rstd = r.alloc((size_t)G * width);
+    t.scale = r.keep((size_t)G * width); t.shift = r.keep((size_t)G * width);
+    t.mean = r.keep((size_t)G * width); t.rstd = r.keep((size_t)G * width);
     t.width = width;
     return t;
 }
 
 struct Gemm {
     CmganGemmArgs a;
+    bool wg = false;
     Gemm(const float* A, long long lda, const float* W, long long sb_tap, long long sb_k, long long sb_n, const float* bias, float* Cout,
          long long ldc, long long M, int N, int Cin) {
         memset(&a, 0, sizeof(a));
@@ -149,8 +209,8 @@ struct Gemm {
         a.mul_y = a.mul_x = a.div_y = a.div_x = 1;
         a.inv_keep = 1.f; a.pro_inv_keep = 1.f; a.alpha = 1.f; a.pro_alpha = 1.f;
     }
-    Gemm& conv(int OH, int OW, int IH, int IW, int mul_x = 1) {
-        a.conv = 1; a.OH = OH; a.OW = OW; a.IH = IH; a.IW = IW; a.mul_x = mul_x;
+    Gemm& conv(int OH, int OW, int IH, int IW, int mul_x = 1, int div_x = 1) {
+        a.conv = 1; a.OH = OH; a.OW = OW; a.IH = IH; a.IW = IW; a.mul_x = mul_x; a.div_x = div_x;
         return *this;
     }
     Gemm& taps(int n, const int* dy, const int* dx) {
@@ -159,8 +219,17 @@ struct Gemm {
         return *this;
     }
     Gemm& residual(const float* R, long long ldr) { a.epi = CMGAN_EPI_DROP_RES; a.R = R; a.ldr = ldr; return *this; }
+    Gemm& drop(unsigned long long seed, unsigned thr, float inv_keep) { a.seed = seed; a.drop_thr = thr; a.inv_keep = inv_keep; return *this; }
+    Gemm& epi(int e, const float* aux, long long ldaux) { a.epi = e; a.aux = aux; a.ldaux = ldaux; return *this; }
+    // weight gradient: accumulates dW (laid out like W: C = dW, ldc = 0) from A and the upstream gradient rows D
+    Gemm& wgrad(const float* D, long long ldd, float* dbias) { wg = true; a.D = D; a.ldd = ldd; a.dbias = dbias; return *this; }
     void run(Run& r) {
         a.precision = r.precision;
+        a.seed_dev = r.seed_dev;
+        if (wg) {
+            if (r.wgrad && r.live()) r.ok(cmgan_gemm_wgrad_f32(&a, r.st));
+            return;
+        }
         if (r.precision == 1 && a.N % 16 == 0 && a.N <= 256 && a.Cin % 32 == 0) {      // scratch for the re-tiled weight (gemm_args.h)
             a.ws_floats = (long long)a.N * a.Cin * a.ntaps;
             a.ws = r.alloc((size_t)a.ws_floats);
@@ -186,31 +255,37 @@ void inst_norm_site(Run& r, const float* x, long long ldx, int G, long long rows
 }
 
 // InstanceNorm2d(affine) + PReLU of a raw (M, 64) tensor, written into dst (generator.py:35-37)
-void norm_prelu_to(Run& r, const float* raw, int G, long long rows, long long rows_per_t, const float* gamma, const float* beta, const float* slope,
+Tabs norm_prelu_to(Run& r, const float* raw, int G, long long rows, long long rows_per_t, const float* gamma, const float* beta, const float* slope,
                    float* dst, long long ldd, double*& sums) {
     Tabs t = make_tabs(r, G, C);
     inst_norm_site(r, raw, C, G, rows, rows_per_t, C, gamma, beta, t, sums);
     if (r.live()) r.ok(cmgan_norm_apply(raw, C, G, rows, C, 1 | (r.precision == 1 ? 16 : 0), t.scale, t.shift, C, slope, dst, ldd, r.st));
+    return t;
 }
 
-// DilatedDenseNet (generator.py:39-47) on the concat buffer cat = [out4 | out3 | out2 | out1 | x]
-void dense_block(Run& r, float* cat, const std::string& p, int B, int T, int Fw, double*& sums) {
+const int W3_DY[3] = {0, 0, 0}, W3_DX[3] = {-1, 0, 1}, W3T_DX[3] = {1, 0, -1};     // (1, 3) convolutions and their data gradients
+
+// DilatedDenseNet (generator.py:39-47) on the concat buffer cat = [out4 | out3 | out2 | out1 | x]; `ds` records the raw outputs and tables
+void dense_block(Run& r, float* cat, const std::string& p, int B, int T, int Fw, double*& sums, DenseSaved* ds = nullptr) {
     const long long M = (long long)B * T * Fw, rows = (long long)T * Fw;
     for (int i = 1; i <= 4; ++i) {
         const int dil = 1 << (i - 1), c0 = (5 - i) * C, Cin = C * i, co = (4 - i) * C;
         const std::string s = std::to_string(i);
-        float* raw = r.alloc((size_t)M * C);
+        float* raw = r.keep((size_t)M * C);
         const int dy[6] = {-dil, -dil, -dil, 0, 0, 0}, dx[6] = {-1, 0, 1, -1, 0, 1};         // tap = kh * 3 + kw, causal in time (generator.py:12-21)
-        Gemm(cat ? cat + c0 : nullptr, CAT, r.w(p + "conv" + s + ".weight"), 1, 6, (long long)Cin * 6, r.w(p + "conv" + s + ".bias"), raw, C, M, C, Cin)
+        Gemm(off(cat, c0), CAT, r.w(p + "conv" + s + ".weight"), 1, 6, (long long)Cin * 6, r.w(p + "conv" + s + ".bias"), raw, C, M, C, Cin)
             .taps(6, dy, dx).conv(T, Fw, T, Fw).run(r);
-        norm_prelu_to(r, raw, B, rows, Fw, r.w(p + "norm" + s + ".weight"), r.w(p + "norm" + s + ".bias"), r.w(p + "prelu" + s + ".weight"),
-                      cat ? cat + co : nullptr, CAT, sums);
+        const Tabs t = norm_prelu_to(r, raw, B, rows, Fw, r.w(p + "norm" + s + ".weight"), r.w(p + "norm" + s + ".bias"), r.w(p + "prelu" + s + ".weight"),
+                                     off(cat, co), CAT, sums);
+        if (ds) { ds->raw[i - 1] = raw; ds->tab[i - 1] = t; }
     }
 }
 
-// 0.5 * FF(LN(x)) + x  (conformer.py:54-72,136-148,211-212)
-float* feed_forward(Run& r, const float* xin, long long M, const std::string& p) {
-    float* out = r.alloc((size_t)M * C);
+// 0.5 * FF(LN(x)) + x  (conformer.py:54-72,136-148,211-212); dropout (training) with the site seeds s1 (hidden layer) and s2 (output)
+float* feed_forward(Run& r, const float* xin, long long M, const std::string& p, unsigned long long s1 = 0, unsigned long long s2 = 0, FfSaved* fs = nullptr) {
+    const unsigned thr = drop_thr(r.training);
+    const float inv = drop_inv(r.training);
+    float* out = r.keep((size_t)M * C);
     if (r.precision == 1) {          // fused kernel: the hidden activation stays on the SM (ffn_fused.cu)
         float* w1p = r.alloc((size_t)4 * C * C);
         float* w2p = r.alloc((size_t)4 * C * C);
@@ -218,38 +293,45 @@ float* feed_forward(Run& r, const float* xin, long long M, const std::string& p)
             r.ok(cmgan_pack_weight(r.w(p + "fn.fn.net.0.weight"), w1p, 0, 1, C, C, 1, 4 * C, r.st));
             r.ok(cmgan_pack_weight(r.w(p + "fn.fn.net.3.weight"), w2p, 0, 1, 4 * C, 4 * C, 1, C, r.st));
             r.ok(cmgan_ffn_fwd(xin, C, M, r.w(p + "fn.norm.weight"), r.w(p + "fn.norm.bias"), w1p, r.w(p + "fn.fn.net.0.bias"), w2p,
-                               r.w(p + "fn.fn.net.3.bias"), 0.5f, 0ull, 0ull, 0u, 1.f, nullptr, out, C, r.st));
+                               r.w(p + "fn.fn.net.3.bias"), 0.5f, s1, s2, thr, inv, r.seed_dev, out, C, r.st));
         }
         return out;
     }
-    float* xn = r.alloc((size_t)M * C);
-    float* stt = r.alloc((size_t)M * 2);
-    float* a = r.alloc((size_t)M * 4 * C);
+    float* xn = r.keep((size_t)M * C);
+    float* stt = r.keep((size_t)M * 2);
+    float* h = fs ? r.keep((size_t)M * 4 * C) : nullptr;           // pre-activation: only the backward reads it
+    float* a = r.keep((size_t)M * 4 * C);
     if (r.live()) r.ok(cmgan_ln_apply(xin, C, M, r.w(p + "fn.norm.weight"), r.w(p + "fn.norm.bias"), nullptr, 0, xn, C, stt, r.precision == 1 ? 1 : 0, r.st));
-    Gemm g1(xn, C, r.w(p + "fn.fn.net.0.weight"), 0, 1, C, r.w(p + "fn.fn.net.0.bias"), nullptr, 4 * C, M, 4 * C, C);
+    Gemm g1(xn, C, r.w(p + "fn.fn.net.0.weight"), 0, 1, C, r.w(p + "fn.fn.net.0.bias"), h, 4 * C, M, 4 * C, C);
     g1.a.epi = CMGAN_EPI_SWISH_DUAL; g1.a.C2 = a; g1.a.ldc2 = 4 * C;
-    g1.run(r);
+    g1.drop(s1, thr, inv).run(r);
     Gemm g2(a, 4 * C, r.w(p + "fn.fn.net.3.weight"), 0, 1, 4 * C, r.w(p + "fn.fn.net.3.bias"), out, C, M, C, 4 * C);
-    g2.residual(xin, C).a.alpha = 0.5f;
+    g2.residual(xin, C).drop(s2, thr, inv).a.alpha = 0.5f;
     g2.run(r);
+    if (fs) { fs->xn = xn; fs->st = stt; fs->h = h; fs->a = a; }
     return out;
 }
 
-// ConformerBlock + the outer TSCB residual (conformer.py:216-222, generator.py:95,97): returns LN(x4) + x in `y`
-void conformer(Run& r, const float* x, float* y, const std::string& p, int B, int T, int F2, int axis) {
+// ConformerBlock + the outer TSCB residual (conformer.py:216-222, generator.py:95,97): returns LN(x4) + x in `y`.
+// Training: dropout at the five sites (seeds from block_id), BatchNorm batch statistics from the depthwise kernel's epilogue sums.
+void conformer(Run& r, const float* x, float* y, const std::string& p, int B, int T, int F2, int axis, int block_id = 0, double** sums = nullptr,
+               ConfSaved* cs = nullptr) {
     const long long M = (long long)B * T * F2;
     const size_t mark = r.top;
     const int rnd = r.precision == 1 ? 1 : 0;
-    float* x1 = feed_forward(r, x, M, p + "ff1.");
+    unsigned long long sd[5] = {0, 0, 0, 0, 0};
+    if (r.training)
+        for (int i = 0; i < 5; ++i) sd[i] = site_seed(r.seed, block_id, i);
+    float* x1 = feed_forward(r, x, M, p + "ff1.", sd[0], sd[1], cs ? &cs->f1 : nullptr);
     // ---- attention (conformer.py:90-133)
-    float* xn2 = r.alloc((size_t)M * C);
-    float* st2 = r.alloc((size_t)M * 2);
+    float* xn2 = r.keep((size_t)M * C);
+    float* st2 = r.keep((size_t)M * 2);
     if (r.live()) r.ok(cmgan_ln_apply(x1, C, M, r.w(p + "attn.norm.weight"), r.w(p + "attn.norm.bias"), nullptr, 0, xn2, C, st2, rnd, r.st));
-    float* qkv = r.alloc((size_t)M * 3 * C);
+    float* qkv = r.keep((size_t)M * 3 * C);
     // to_q and to_kv are adjacent in the parameter block: one (192, 64) projection
     Gemm(xn2, C, r.w(p + "attn.fn.to_q.weight"), 0, 1, C, nullptr, qkv, 3 * C, M, 3 * C, C).run(r);
-    float* ctx = r.alloc((size_t)M * C);
-    float* lse = r.alloc((size_t)M * 4);
+    float* ctx = r.keep((size_t)M * C);
+    float* lse = r.keep((size_t)M * 4);
     if (r.live()) {
         const float* E = r.w(p + "attn.fn.rel_pos_emb.weight");
         if (r.frames)
@@ -258,92 +340,115 @@ void conformer(Run& r, const float* x, float* y, const std::string& p, int B, in
         else
             r.ok(r.precision == 1 ? cmgan_attention_fwd_tf32(qkv, E, B, T, F2, axis, ctx, lse, r.st) : cmgan_attention_fwd(qkv, E, B, T, F2, axis, ctx, lse, r.st));
     }
-    float* x2 = r.alloc((size_t)M * C);
-    Gemm(ctx, C, r.w(p + "attn.fn.to_out.weight"), 0, 1, C, r.w(p + "attn.fn.to_out.bias"), x2, C, M, C, C).residual(x1, C).run(r);
+    float* x2 = r.keep((size_t)M * C);
+    Gemm(ctx, C, r.w(p + "attn.fn.to_out.weight"), 0, 1, C, r.w(p + "attn.fn.to_out.bias"), x2, C, M, C, C).residual(x1, C)
+        .drop(sd[2], drop_thr(r.training), drop_inv(r.training)).run(r);
     // ---- convolution module (conformer.py:160-173)
-    float* xn3 = r.alloc((size_t)M * C);
-    float* st3 = r.alloc((size_t)M * 2);
+    float* xn3 = r.keep((size_t)M * C);
+    float* st3 = r.keep((size_t)M * 2);
     if (r.live()) r.ok(cmgan_ln_apply(x2, C, M, r.w(p + "conv.net.0.weight"), r.w(p + "conv.net.0.bias"), nullptr, 0, xn3, C, st3, rnd, r.st));
-    float* g = r.alloc((size_t)M * 4 * C);
+    float* g = r.keep((size_t)M * 4 * C);
     Gemm(xn3, C, r.w(p + "conv.net.2.weight"), 0, 1, C, r.w(p + "conv.net.2.bias"), g, 4 * C, M, 4 * C, C).run(r);
-    float* d = r.alloc((size_t)M * 2 * C);
+    float* d = r.keep((size_t)M * 2 * C);
     Tabs bn = make_tabs(r, 1, 2 * C);
-    float* dsw = r.alloc((size_t)M * 2 * C);
+    float* dsw = r.keep((size_t)M * 2 * C);
+    double* bs = nullptr;        // training: per-channel sum and sum of squares of d, from the depthwise kernel's epilogue
+    if (r.training) { bs = *sums; *sums += 2 * C * 2; }
     if (r.live()) {
+        float* rmean = const_cast<float*>(r.w(p + "conv.net.5.running_mean"));
+        float* rvar = const_cast<float*>(r.w(p + "conv.net.5.running_var"));
         if (r.frames)
             r.ok(cmgan_glu_dwconv_fwd_ragged(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, r.frames, d, r.st));
         else
-            r.ok(cmgan_glu_dwconv_fwd(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, d, nullptr, r.st));
-        // eval: BatchNorm1d folds to scale / shift from the running statistics (mode 1; they are only read)
-        r.ok(cmgan_norm_finalize(nullptr, M, 1, 2 * C, 1, r.w(p + "conv.net.5.weight"), r.w(p + "conv.net.5.bias"),
-                                 const_cast<float*>(r.w(p + "conv.net.5.running_mean")), const_cast<float*>(r.w(p + "conv.net.5.running_var")), 0.1f,
-                                 bn.scale, bn.shift, bn.mean, bn.rstd, 2 * C, r.st));
+            r.ok(cmgan_glu_dwconv_fwd(g, r.w(p + "conv.net.4.conv.weight"), r.w(p + "conv.net.4.conv.bias"), B, T, F2, axis, d, bs, r.st));
+        if (r.training)     // batch statistics; the running statistics are updated in place (momentum 0.1, unbiased variance)
+            r.ok(cmgan_norm_finalize(bs, M, 1, 2 * C, 0, r.w(p + "conv.net.5.weight"), r.w(p + "conv.net.5.bias"), rmean, rvar, 0.1f,
+                                     bn.scale, bn.shift, bn.mean, bn.rstd, 2 * C, r.st));
+        else                // eval: BatchNorm1d folds to scale / shift from the running statistics (mode 1; they are only read)
+            r.ok(cmgan_norm_finalize(nullptr, M, 1, 2 * C, 1, r.w(p + "conv.net.5.weight"), r.w(p + "conv.net.5.bias"), rmean, rvar, 0.1f,
+                                     bn.scale, bn.shift, bn.mean, bn.rstd, 2 * C, r.st));
         r.ok(cmgan_norm_apply(d, 2 * C, 1, M, 2 * C, 2 | (16 * rnd), bn.scale, bn.shift, 2 * C, nullptr, dsw, 2 * C, r.st));
     }
-    float* x3 = r.alloc((size_t)M * C);
+    float* x3 = r.keep((size_t)M * C);
     Gemm(dsw, 2 * C, r.w(p + "conv.net.7.weight"), 0, 1, 2 * C, r.w(p + "conv.net.7.bias"), x3, C, M, C, 2 * C).residual(x2, C).run(r);
     // ---- second feed-forward, post norm, outer residual
-    float* x4 = feed_forward(r, x3, M, p + "ff2.");
-    float* st5 = r.alloc((size_t)M * 2);
+    float* x4 = feed_forward(r, x3, M, p + "ff2.", sd[3], sd[4], cs ? &cs->f2 : nullptr);
+    float* st5 = r.keep((size_t)M * 2);
     if (r.live()) r.ok(cmgan_ln_apply(x4, C, M, r.w(p + "post_norm.weight"), r.w(p + "post_norm.bias"), x, C, y, C, st5, 0, r.st));
-    r.top = mark;            // everything but `y` (owned by the caller) is released
+    if (cs) {
+        cs->x = x; cs->x1 = x1; cs->xn2 = xn2; cs->st2 = st2; cs->qkv = qkv; cs->ctx = ctx; cs->lse = lse; cs->x2 = x2; cs->xn3 = xn3; cs->st3 = st3;
+        cs->g = g; cs->d = d; cs->dsw = dsw; cs->bn = bn; cs->x3 = x3; cs->x4 = x4; cs->st5 = st5;
+    }
+    r.top = mark;            // everything but `y` (owned by the caller) and the saved activations is released
 }
+
+const char* conformer_name(int k) {         // k = (i - 1) * 2 + axis: the block_id of conformer_block._site_seed
+    static const char* n[8] = {"TSCB_1.time_conformer.", "TSCB_1.freq_conformer.", "TSCB_2.time_conformer.", "TSCB_2.freq_conformer.",
+                               "TSCB_3.time_conformer.", "TSCB_3.freq_conformer.", "TSCB_4.time_conformer.", "TSCB_4.freq_conformer."};
+    return n[k];
+}
+const char* const DEC_NAMES[2] = {"mask_decoder.", "complex_decoder."};
+
+// statistics scratch of one pass (network._sums_size): every InstanceNorm site, plus the BatchNorm sums of the conformers in training
+size_t sums_size(int B, bool training) { return (size_t)(16 * C + 2) * B * 2 + 64 + (training ? 8 * 2 * C * 2 : 0); }
 
 void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, float* fr, float* fi) {
     const int F2 = (F - 1) / 2 + 1;
     const long long M = (long long)B * T * F, M2 = (long long)B * T * F2;
-    const size_t n_sums = (size_t)(16 * C + 2) * B * 2 + 64;
+    Saved* sv = r.sv;
+    const size_t n_sums = sums_size(B, r.training);
     double* sums0 = r.alloc<double>(n_sums);
     double* sums = sums0;
     if (r.live()) {
         cudaError_t e = cudaMemsetAsync(sums0, 0, n_sums * sizeof(double), r.st);
         if (e != cudaSuccess) { cmgan_set_error("cmgan_tscnet_fwd: cudaMemsetAsync: %s", cudaGetErrorString(e)); r.rc = -1; }
     }
-    float* hA = r.alloc((size_t)M2 * C);          // TSCB activations ping-pong between these two
-    float* hB = r.alloc((size_t)M2 * C);
+    // TSCB activations ping-pong between these two; when saving, every block's input is kept instead
+    float* hA = sv ? r.keep((size_t)M2 * C) : r.alloc((size_t)M2 * C);
+    float* hB = sv ? nullptr : r.alloc((size_t)M2 * C);
     // ---- dense encoder (generator.py:50-69)
     {
         const size_t mark = r.top;
         const std::string pe = "dense_encoder.";
-        float* catE = r.alloc((size_t)M * CAT);
-        float* raw0 = r.alloc((size_t)M * C);
+        float* catE = r.keep((size_t)M * CAT);
+        float* raw0 = r.keep((size_t)M * C);
         if (r.live()) r.ok(cmgan_head_conv(x, sxb, sxc, sxt, sxf, B, T, F, r.w(pe + "conv_1.0.weight"), r.w(pe + "conv_1.0.bias"), raw0, C, r.st));
-        norm_prelu_to(r, raw0, B, (long long)T * F, F, r.w(pe + "conv_1.1.weight"), r.w(pe + "conv_1.1.bias"), r.w(pe + "conv_1.2.weight"),
-                      catE ? catE + 4 * C : nullptr, CAT, sums);
-        dense_block(r, catE, pe + "dilated_dense.", B, T, F, sums);
-        float* e2 = r.alloc((size_t)M2 * C);
-        const int dy[3] = {0, 0, 0}, dx[3] = {-1, 0, 1};
-        Gemm(catE, CAT, r.w(pe + "conv_2.0.weight"), 1, 3, 3 * C, r.w(pe + "conv_2.0.bias"), e2, C, M2, C, C).taps(3, dy, dx).conv(T, F2, T, F, 2).run(r);
+        const Tabs t0 = norm_prelu_to(r, raw0, B, (long long)T * F, F, r.w(pe + "conv_1.1.weight"), r.w(pe + "conv_1.1.bias"),
+                                      r.w(pe + "conv_1.2.weight"), off(catE, 4 * C), CAT, sums);
+        dense_block(r, catE, pe + "dilated_dense.", B, T, F, sums, sv ? &sv->enc : nullptr);
+        float* e2 = r.keep((size_t)M2 * C);
+        Gemm(catE, CAT, r.w(pe + "conv_2.0.weight"), 1, 3, 3 * C, r.w(pe + "conv_2.0.bias"), e2, C, M2, C, C).taps(3, W3_DY, W3_DX).conv(T, F2, T, F, 2).run(r);
         Tabs t2 = make_tabs(r, B, C);
         inst_norm_site(r, e2, C, B, (long long)T * F2, F2, C, r.w(pe + "conv_2.1.weight"), r.w(pe + "conv_2.1.bias"), t2, sums);
         if (r.live()) r.ok(cmgan_norm_apply(e2, C, B, (long long)T * F2, C, 1, t2.scale, t2.shift, C, r.w(pe + "conv_2.2.weight"), hA, C, r.st));
+        if (sv) { sv->catE = catE; sv->raw0 = raw0; sv->tab0 = t0; sv->e2 = e2; sv->tab2 = t2; }
         r.top = mark;
     }
     // ---- 4 x TSCB (generator.py:92-99): time conformer then frequency conformer on the same rows
     float *h = hA, *hn = hB;
-    for (int i = 1; i <= 4; ++i)
-        for (int axis = 0; axis < 2; ++axis) {
-            conformer(r, h, hn, "TSCB_" + std::to_string(i) + (axis == 0 ? ".time_conformer." : ".freq_conformer."), B, T, F2, axis);
-            float* t = h; h = hn; hn = t;
-        }
+    for (int k = 0; k < 8; ++k) {
+        if (sv) hn = r.keep((size_t)M2 * C);
+        conformer(r, h, hn, conformer_name(k), B, T, F2, k % 2, k, &sums, sv ? &sv->conf[k] : nullptr);
+        float* t = h; h = hn; hn = t;
+    }
     // ---- decoders (generator.py:122-156)
     float* sp[2];
-    const char* names[2] = {"mask_decoder.", "complex_decoder."};
     for (int dd = 0; dd < 2; ++dd) {
-        const std::string pd = names[dd];
-        sp[dd] = r.alloc((size_t)M2 * 2 * C);          // (B, T, 2 F2, 64): the sub-pixel shuffle is a reinterpretation
+        const std::string pd = DEC_NAMES[dd];
+        sp[dd] = r.keep((size_t)M2 * 2 * C);          // (B, T, 2 F2, 64): the sub-pixel shuffle is a reinterpretation
         const size_t mark = r.top;
-        float* cat = r.alloc((size_t)M2 * CAT);
+        float* cat = r.keep((size_t)M2 * CAT);
         if (r.live()) r.ok(cmgan_copy_rows_operand(h, C, cat + 4 * C, CAT, M2, C, r.st));
-        dense_block(r, cat, pd + "dense_block.", B, T, F2, sums);
-        const int dy[3] = {0, 0, 0}, dx[3] = {-1, 0, 1};
+        dense_block(r, cat, pd + "dense_block.", B, T, F2, sums, sv ? &sv->dec[dd] : nullptr);
         Gemm(cat, CAT, r.w(pd + "sub_pixel.conv.weight"), 1, 3, 3 * C, r.w(pd + "sub_pixel.conv.bias"), sp[dd], 2 * C, M2, 2 * C, C)
-            .taps(3, dy, dx).conv(T, F2, T, F2).run(r);
+            .taps(3, W3_DY, W3_DX).conv(T, F2, T, F2).run(r);
+        if (sv) { sv->cat[dd] = cat; sv->sp[dd] = sp[dd]; }
         r.top = mark;
     }
     const std::string pm = "mask_decoder.", pc = "complex_decoder.";
-    float* m1 = r.alloc((size_t)M);
+    float* m1 = r.keep((size_t)M);
     Tabs tabM = make_tabs(r, B, 1), tabC = make_tabs(r, B, C);
+    if (sv) { sv->m1 = m1; sv->tabM = tabM; sv->tabC = tabC; }
     float* cplx = r.alloc((size_t)M * 2);
     if (r.live()) r.ok(cmgan_rowdot_fwd(sp[0], B, T, F, 1, nullptr, nullptr, nullptr, r.w(pm + "conv_1.weight"), r.w(pm + "conv_1.bias"), m1, r.st));
     inst_norm_site(r, m1, 1, B, (long long)T * F, F, 1, r.w(pm + "norm.weight"), r.w(pm + "norm.bias"), tabM, sums);
@@ -354,6 +459,236 @@ void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt
                              r.w(pm + "prelu_out.weight"), x, sxb, sxc, sxt, sxf, cplx, B, T, F, fr, fi, r.st));
     }
     if ((size_t)(sums - sums0) > n_sums && r.rc == 0) { cmgan_set_error("cmgan_tscnet_fwd: statistics scratch exhausted"); r.rc = -1; }
+}
+
+// ==================================================================================== backward (network.tscnet_bwd, conformer_block.conformer_bwd)
+// The launch sequence of the Python walk on one stream (ops.WGRAD_STREAM = ops.AUX_STREAM = None, no weight-pack cache, ATTN_BWD_WS off).
+
+// InstanceNorm / BatchNorm (+ PReLU) backward of one site (conformer_block._norm_bwd); `operand`: dx feeds tensor-core contractions
+void norm_bwd(Run& r, const float* x, long long ldx, const float* dact, long long ldd, int G, long long rows, int Cn, int act, int batch_stats,
+              const Tabs& t, const float* slope, float* dx, long long lddx, float* dgamma, float* dbeta, float* dslope, double*& sums, bool operand) {
+    double* s = sums;
+    sums += (size_t)G * Cn * 2;
+    if (!r.live()) return;
+    r.ok(cmgan_norm_bwd_reduce(x, ldx, dact, ldd, G, rows, Cn, act, t.scale, t.shift, t.mean, t.rstd, t.width, slope, s, dslope, r.st));
+    r.ok(cmgan_norm_bwd_apply(x, ldx, dact, ldd, G, rows, Cn, act | (operand && r.precision == 1 ? 16 : 0), batch_stats, t.scale, t.shift, t.mean,
+                              t.rstd, t.width, slope, s, dx, lddx, dgamma, dbeta, r.st));
+}
+
+// LayerNorm backward (+ residual gradients); with dz also the dropout-scaled copy dz = zalpha * mask(zseed) * dx that enters the next branch
+void ln_bwd(Run& r, long long M, const float* dy, const float* x, const float* st, const std::string& name, const float* res, const float* res2,
+            float* dx, float* dz = nullptr, float zalpha = 0.f, unsigned long long zseed = 0) {
+    if (!r.live()) return;
+    const float* gam = r.w(name + ".weight");
+    float *dg = r.g(name + ".weight"), *db = r.g(name + ".bias");
+    if (!dz)
+        r.ok(cmgan_ln_bwd(dy, C, x, C, st, gam, M, res, res ? C : 0, res2, res2 ? C : 0, dx, C, dg, db, r.st));
+    else
+        r.ok(cmgan_ln_bwd_drop(dy, C, x, C, st, gam, M, res, res ? C : 0, res2, res2 ? C : 0, dx, C, dg, db, dz, C, zalpha, zseed, drop_thr(r.training),
+                               drop_inv(r.training), r.seed_dev, r.st));
+}
+
+// out = xin + 0.5 * drop2(W2 a + b2), a = swish(h) * drop1, h = W1 LN(xin) + b1;  dz = 0.5 * drop2-mask * dout  ->  dx (+ res2)
+void feed_forward_bwd(Run& r, long long M, const std::string& p, const FfSaved& f, const float* xin, const float* dout, const float* dz,
+                      const float* res2, unsigned long long s1, float* dx) {
+    const size_t mark = r.top;
+    const float *W1 = r.w(p + "fn.fn.net.0.weight"), *W2 = r.w(p + "fn.fn.net.3.weight");
+    if (r.precision == 1) {      // hidden activation recomputed, dh formed in the same kernel; it leaves a, dh and xn for the weight gradients
+        float* w1p = r.alloc((size_t)4 * C * C);
+        float* w2tp = r.alloc((size_t)4 * C * C);
+        float* w1tp = r.alloc((size_t)4 * C * C);
+        float* a = r.alloc((size_t)M * 4 * C);
+        float* dh = r.alloc((size_t)M * 4 * C);
+        float* xn = r.alloc((size_t)M * C);
+        float* ws = r.alloc((size_t)M * (2 + C));
+        if (r.live()) {
+            r.ok(cmgan_pack_weight(W1, w1p, 0, 1, C, C, 1, 4 * C, r.st));
+            r.ok(cmgan_pack_weight(W2, w2tp, 0, 4 * C, 1, C, 1, 4 * C, r.st));
+            r.ok(cmgan_pack_weight(W1, w1tp, 0, C, 1, 4 * C, 1, C, r.st));
+            r.ok(cmgan_ffn_bwd(xin, C, dz, C, dout, C, res2, res2 ? C : 0, M, r.w(p + "fn.norm.weight"), r.w(p + "fn.norm.bias"), w1p,
+                               r.w(p + "fn.fn.net.0.bias"), w2tp, w1tp, s1, drop_thr(r.training), drop_inv(r.training), r.seed_dev, dx, C, a, dh, xn,
+                               r.g(p + "fn.norm.weight"), r.g(p + "fn.norm.bias"), ws, r.st));
+        }
+        Gemm(a, 4 * C, nullptr, 0, 1, 4 * C, nullptr, r.g(p + "fn.fn.net.3.weight"), 0, M, C, 4 * C).wgrad(dz, C, r.g(p + "fn.fn.net.3.bias")).run(r);
+        Gemm(xn, C, nullptr, 0, 1, C, nullptr, r.g(p + "fn.fn.net.0.weight"), 0, M, 4 * C, C).wgrad(dh, 4 * C, r.g(p + "fn.fn.net.0.bias")).run(r);
+        r.top = mark;
+        return;
+    }
+    float* dh = r.alloc((size_t)M * 4 * C);
+    Gemm(dz, C, W2, 0, 4 * C, 1, nullptr, dh, 4 * C, M, 4 * C, C).epi(CMGAN_EPI_DSWISH_DROP, f.h, 4 * C)
+        .drop(s1, drop_thr(r.training), drop_inv(r.training)).run(r);
+    Gemm(f.a, 4 * C, nullptr, 0, 1, 4 * C, nullptr, r.g(p + "fn.fn.net.3.weight"), 0, M, C, 4 * C).wgrad(dz, C, r.g(p + "fn.fn.net.3.bias")).run(r);
+    float* dln = r.alloc((size_t)M * C);
+    Gemm(dh, 4 * C, W1, 0, C, 1, nullptr, dln, C, M, C, 4 * C).run(r);
+    Gemm(f.xn, C, nullptr, 0, 1, C, nullptr, r.g(p + "fn.fn.net.0.weight"), 0, M, 4 * C, C).wgrad(dh, 4 * C, r.g(p + "fn.fn.net.0.bias")).run(r);
+    ln_bwd(r, M, dln, xin, f.st, p + "fn.norm", dout, res2, dx);
+    r.top = mark;
+}
+
+// gradient of conformer(): dy (M, 64) -> dx (M, 64)
+void conformer_bwd(Run& r, const ConfSaved& s, const float* dy, float* dx, const std::string& p, int B, int T, int F2, int axis, int block_id,
+                   double*& sums) {
+    const long long M = (long long)B * T * F2;
+    const size_t mark = r.top;
+    unsigned long long sd[5];
+    for (int i = 0; i < 5; ++i) sd[i] = site_seed(r.seed, block_id, i);
+    // y = LN(x4) * g + b + x
+    float* dx4 = r.alloc((size_t)M * C);
+    float* dz4 = r.alloc((size_t)M * C);
+    ln_bwd(r, M, dy, s.x4, s.st5, p + "post_norm", nullptr, nullptr, dx4, dz4, 0.5f, sd[4]);
+    float* dx3 = r.alloc((size_t)M * C);
+    feed_forward_bwd(r, M, p + "ff2.", s.f2, s.x3, dx4, dz4, nullptr, sd[3], dx3);
+    // ---- convolution module: x3 = x2 + W7 swish(bn(d)) + b7
+    float* dbn = r.alloc((size_t)M * 2 * C);
+    const float* dx3_op = dx3;
+    if (r.precision == 1) {      // dx3 also carries the residual gradient at full precision: the tensor-core operand is a rounded copy
+        float* t = r.alloc((size_t)M * C);
+        if (r.live()) r.ok(cmgan_copy_rows_operand(dx3, C, t, C, M, C, r.st));
+        dx3_op = t;
+    }
+    Gemm gb(dx3_op, C, r.w(p + "conv.net.7.weight"), 0, 2 * C, 1, nullptr, dbn, 2 * C, M, 2 * C, C);
+    gb.epi(CMGAN_EPI_DBNSWISH, s.d, 2 * C);
+    gb.a.e0 = s.bn.scale; gb.a.e1 = s.bn.shift;
+    gb.run(r);
+    Gemm(s.dsw, 2 * C, nullptr, 0, 1, 2 * C, nullptr, r.g(p + "conv.net.7.weight"), 0, M, C, 2 * C).wgrad(dx3, C, r.g(p + "conv.net.7.bias")).run(r);
+    float* dd = r.alloc((size_t)M * 2 * C);
+    norm_bwd(r, s.d, 2 * C, dbn, 2 * C, 1, M, 2 * C, 0, r.training ? 1 : 0, s.bn, nullptr, dd, 2 * C, r.g(p + "conv.net.5.weight"),
+             r.g(p + "conv.net.5.bias"), nullptr, sums, false);
+    float* dg = r.alloc((size_t)M * 4 * C);
+    if (r.live())
+        r.ok(cmgan_glu_dwconv_bwd(s.g, dd, r.w(p + "conv.net.4.conv.weight"), B, T, F2, axis, dg, r.g(p + "conv.net.4.conv.weight"),
+                                  r.g(p + "conv.net.4.conv.bias"), r.st));
+    float* dln3 = r.alloc((size_t)M * C);
+    Gemm(dg, 4 * C, r.w(p + "conv.net.2.weight"), 0, C, 1, nullptr, dln3, C, M, C, 4 * C).run(r);
+    Gemm(s.xn3, C, nullptr, 0, 1, C, nullptr, r.g(p + "conv.net.2.weight"), 0, M, 4 * C, C).wgrad(dg, 4 * C, r.g(p + "conv.net.2.bias")).run(r);
+    float* dx2 = r.alloc((size_t)M * C);
+    float* dz2 = r.training ? r.alloc((size_t)M * C) : dx2;     // attention dropout: the to_out branch sees mask * dx2
+    ln_bwd(r, M, dln3, s.x2, s.st3, p + "conv.net.0", dx3, nullptr, dx2, r.training ? dz2 : nullptr, 1.f, sd[2]);
+    // ---- attention: x2 = x1 + drop(ctx Wo^T + bo)
+    float* dctx = r.alloc((size_t)M * C);
+    Gemm(dz2, C, r.w(p + "attn.fn.to_out.weight"), 0, C, 1, nullptr, dctx, C, M, C, C).run(r);
+    Gemm(s.ctx, C, nullptr, 0, 1, C, nullptr, r.g(p + "attn.fn.to_out.weight"), 0, M, C, C).wgrad(dz2, C, r.g(p + "attn.fn.to_out.bias")).run(r);
+    float* dqkv = r.alloc((size_t)M * 3 * C);
+    float* delta = r.alloc((size_t)M * 4);
+    if (r.live()) {
+        const float* E = r.w(p + "attn.fn.rel_pos_emb.weight");
+        float* dE = r.g(p + "attn.fn.rel_pos_emb.weight");
+        r.ok(r.precision == 1 ? cmgan_attention_bwd_tf32_ws(s.qkv, E, s.ctx, dctx, s.lse, B, T, F2, axis, delta, dqkv, dE, 7, nullptr, 0, r.st)
+                              : cmgan_attention_bwd(s.qkv, E, s.ctx, dctx, s.lse, B, T, F2, axis, delta, dqkv, dE, r.st));
+    }
+    // to_q and to_kv (and their gradients) are adjacent in the blocks: one (192, 64) projection
+    float* dln2 = r.alloc((size_t)M * C);
+    Gemm(dqkv, 3 * C, r.w(p + "attn.fn.to_q.weight"), 0, C, 1, nullptr, dln2, C, M, C, 3 * C).run(r);
+    Gemm(s.xn2, C, nullptr, 0, 1, C, nullptr, r.g(p + "attn.fn.to_q.weight"), 0, M, 3 * C, C).wgrad(dqkv, 3 * C, nullptr).run(r);
+    float* dx1 = r.alloc((size_t)M * C);
+    float* dz1 = r.alloc((size_t)M * C);
+    ln_bwd(r, M, dln2, s.x1, s.st2, p + "attn.norm", dx2, nullptr, dx1, dz1, 0.5f, sd[1]);
+    // ---- first feed-forward; the outer residual adds dy
+    feed_forward_bwd(r, M, p + "ff1.", s.f1, s.x, dx1, dz1, dy, sd[0], dx);
+    r.top = mark;
+}
+
+// dcat slot 0 holds the gradient wrt act(out4); on return dcat slot 4 holds the gradient wrt the block input (network.dense_block_bwd)
+void dense_block_bwd(Run& r, const float* cat, const DenseSaved& s, float* dcat, const std::string& p, int B, int T, int Fw, double*& sums) {
+    const long long M = (long long)B * T * Fw, rows = (long long)T * Fw;
+    for (int i = 4; i >= 1; --i) {
+        const int dil = 1 << (i - 1), c0 = (5 - i) * C, Cin = C * i, co = (4 - i) * C;
+        const std::string n = std::to_string(i);
+        const size_t mark = r.top;
+        float* draw = r.alloc((size_t)M * C);
+        norm_bwd(r, s.raw[i - 1], C, off(dcat, co), CAT, B, rows, C, 1, 1, s.tab[i - 1], r.w(p + "prelu" + n + ".weight"), draw, C,
+                 r.g(p + "norm" + n + ".weight"), r.g(p + "norm" + n + ".bias"), r.g(p + "prelu" + n + ".weight"), sums, true);
+        const int dy[6] = {-dil, -dil, -dil, 0, 0, 0}, dx[6] = {-1, 0, 1, -1, 0, 1};
+        const int ndy[6] = {dil, dil, dil, 0, 0, 0}, ndx[6] = {1, 0, -1, 1, 0, -1};
+        Gemm(off(cat, c0), CAT, nullptr, 1, 6, (long long)Cin * 6, nullptr, r.g(p + "conv" + n + ".weight"), 0, M, C, Cin).taps(6, dy, dx)
+            .conv(T, Fw, T, Fw).wgrad(draw, C, r.g(p + "conv" + n + ".bias")).run(r);
+        Gemm dg(draw, C, r.w(p + "conv" + n + ".weight"), 1, (long long)Cin * 6, 6, nullptr, off(dcat, c0), CAT, M, Cin, C);
+        dg.taps(6, ndy, ndx).conv(T, Fw, T, Fw).a.epi = i == 4 ? CMGAN_EPI_NONE : CMGAN_EPI_ACC;
+        dg.run(r);
+        r.top = mark;
+    }
+}
+
+// dfr / dfi (B, 1, T, F) with strides (sgb, sgt, sgf), null = zero; dx (B, 2, T, F) contiguous or null
+void backward(Run& r, const Saved& sv, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, const float* dfr,
+              const float* dfi, long long sgb, long long sgt, long long sgf, float* dx) {
+    const int F2 = (F - 1) / 2 + 1;
+    const long long M = (long long)B * T * F, M2 = (long long)B * T * F2;
+    const size_t n_sums = sums_size(B, true);
+    double* sums0 = r.alloc<double>(n_sums);
+    double* sums = sums0;
+    float* zero = r.alloc((size_t)M);            // stands in for a null dfr / dfi (laid out with the given strides: span <= B T F, checked on entry)
+    if (r.live()) {
+        cudaError_t e = cudaMemsetAsync(sums0, 0, n_sums * sizeof(double), r.st);
+        if (e == cudaSuccess && (!dfr || !dfi)) e = cudaMemsetAsync(zero, 0, (size_t)M * sizeof(float), r.st);
+        if (e != cudaSuccess) { cmgan_set_error("cmgan_tscnet_bwd: cudaMemsetAsync: %s", cudaGetErrorString(e)); r.rc = -1; }
+    }
+    if (!dfr) dfr = zero;
+    if (!dfi) dfi = zero;
+    const std::string pm = "mask_decoder.", pc = "complex_decoder.", pe = "dense_encoder.";
+    // ---- tails: final = mask * x + cplx (generator.py:136-139,150,191-196)
+    float* dsp[2] = {r.alloc((size_t)M2 * 2 * C), r.alloc((size_t)M2 * 2 * C)};
+    float *dh = r.alloc((size_t)M2 * C), *dh2 = r.alloc((size_t)M2 * C);      // TSCB gradients ping-pong between these two
+    {
+        const size_t mark = r.top;
+        float* dcplx = r.alloc((size_t)M * 2);
+        float* dz = r.alloc((size_t)M);
+        if (r.live())
+            r.ok(cmgan_recombine_bwd(sv.m1, sv.tabM.scale, sv.tabM.shift, r.w(pm + "prelu.weight"), r.w(pm + "final_conv.weight"), r.w(pm + "final_conv.bias"),
+                                     r.w(pm + "prelu_out.weight"), x, sxb, sxc, sxt, sxf, dfr, dfi, sgb, sgt, sgf, B, T, F, dcplx, dz, r.g(pm + "prelu_out.weight"),
+                                     r.g(pm + "final_conv.weight"), r.g(pm + "final_conv.bias"), r.st));
+        float* dm1 = r.alloc((size_t)M);
+        norm_bwd(r, sv.m1, 1, dz, 1, B, (long long)T * F, 1, 1, 1, sv.tabM, r.w(pm + "prelu.weight"), dm1, 1, r.g(pm + "norm.weight"), r.g(pm + "norm.bias"),
+                 r.g(pm + "prelu.weight"), sums, false);
+        if (r.live()) {
+            r.ok(cmgan_rowdot_bwd(sv.sp[0], B, T, F, 1, nullptr, nullptr, nullptr, r.w(pm + "conv_1.weight"), dm1, dsp[0], r.g(pm + "conv_1.weight"),
+                                  r.g(pm + "conv_1.bias"), r.st));
+            r.ok(cmgan_copy_rows_operand(dsp[0], 2 * C, dsp[0], 2 * C, M2, 2 * C, r.st));      // operand of the sub-pixel convolution's gradient GEMMs
+        }
+        float* dactc = r.alloc((size_t)M2 * 2 * C);
+        if (r.live())
+            r.ok(cmgan_rowdot_bwd(sv.sp[1], B, T, F, 2, sv.tabC.scale, sv.tabC.shift, r.w(pc + "prelu.weight"), r.w(pc + "conv.weight"), dcplx, dactc,
+                                  r.g(pc + "conv.weight"), r.g(pc + "conv.bias"), r.st));
+        norm_bwd(r, sv.sp[1], C, dactc, C, B, (long long)T * 2 * F2, C, 1, 1, sv.tabC, r.w(pc + "prelu.weight"), dsp[1], C, r.g(pc + "norm.weight"),
+                 r.g(pc + "norm.bias"), r.g(pc + "prelu.weight"), sums, true);
+        r.top = mark;
+    }
+    // ---- decoders: sub-pixel convolution, dense block; both add into the gradient of the last TSCB's output
+    for (int dd = 0; dd < 2; ++dd) {
+        const std::string pd = DEC_NAMES[dd];
+        const size_t mark = r.top;
+        float* dcat = r.alloc((size_t)M2 * CAT);
+        Gemm(sv.cat[dd], CAT, nullptr, 1, 3, 3 * C, nullptr, r.g(pd + "sub_pixel.conv.weight"), 0, M2, 2 * C, C).taps(3, W3_DY, W3_DX).conv(T, F2, T, F2)
+            .wgrad(dsp[dd], 2 * C, r.g(pd + "sub_pixel.conv.bias")).run(r);
+        Gemm(dsp[dd], 2 * C, r.w(pd + "sub_pixel.conv.weight"), 1, 3 * C, 3, nullptr, dcat, CAT, M2, C, 2 * C).taps(3, W3_DY, W3T_DX).conv(T, F2, T, F2).run(r);
+        dense_block_bwd(r, sv.cat[dd], sv.dec[dd], dcat, pd + "dense_block.", B, T, F2, sums);
+        if (r.live()) r.ok((dd == 0 ? cmgan_copy_rows : cmgan_add_rows)(dcat + 4 * C, CAT, dh, C, M2, C, r.st));
+        r.top = mark;
+    }
+    // ---- TSCBs in reverse
+    for (int k = 7; k >= 0; --k) {
+        conformer_bwd(r, sv.conf[k], dh, dh2, conformer_name(k), B, T, F2, k % 2, k, sums);
+        float* t = dh; dh = dh2; dh2 = t;
+    }
+    // ---- encoder
+    float* de2 = r.alloc((size_t)M2 * C);
+    norm_bwd(r, sv.e2, C, dh, C, B, (long long)T * F2, C, 1, 1, sv.tab2, r.w(pe + "conv_2.2.weight"), de2, C, r.g(pe + "conv_2.1.weight"),
+             r.g(pe + "conv_2.1.bias"), r.g(pe + "conv_2.2.weight"), sums, true);
+    Gemm(sv.catE, CAT, nullptr, 1, 3, 3 * C, nullptr, r.g(pe + "conv_2.0.weight"), 0, M2, C, C).taps(3, W3_DY, W3_DX).conv(T, F2, T, F, 2)
+        .wgrad(de2, C, r.g(pe + "conv_2.0.bias")).run(r);
+    float* dcatE = r.alloc((size_t)M * CAT);
+    Gemm(de2, C, r.w(pe + "conv_2.0.weight"), 1, 3 * C, 3, nullptr, dcatE, CAT, M, C, C).taps(3, W3_DY, W3T_DX).conv(T, F, T, F2, 1, 2).run(r);
+    dense_block_bwd(r, sv.catE, sv.enc, dcatE, pe + "dilated_dense.", B, T, F, sums);
+    float* draw1 = r.alloc((size_t)M * C);
+    norm_bwd(r, sv.raw0, C, off(dcatE, 4 * C), CAT, B, (long long)T * F, C, 1, 1, sv.tab0, r.w(pe + "conv_1.2.weight"), draw1, C,
+             r.g(pe + "conv_1.1.weight"), r.g(pe + "conv_1.1.bias"), r.g(pe + "conv_1.2.weight"), sums, false);
+    if (r.wgrad && r.live())
+        r.ok(cmgan_head_conv_wgrad(x, sxb, sxc, sxt, sxf, B, T, F, draw1, C, r.g(pe + "conv_1.0.weight"), r.g(pe + "conv_1.0.bias"), r.st));
+    if (dx && r.live())         // final = mask x + cplx and the head reads [|x|, re, im]: one pass over draw1 and the recomputed mask
+        r.ok(cmgan_tscnet_input_grad(sv.m1, sv.tabM.scale, sv.tabM.shift, r.w(pm + "prelu.weight"), r.w(pm + "final_conv.weight"),
+                                     r.w(pm + "final_conv.bias"), r.w(pm + "prelu_out.weight"), x, sxb, sxc, sxt, sxf, dfr, dfi, sgb, sgt, sgf, draw1, C,
+                                     r.w(pe + "conv_1.0.weight"), B, T, F, dx, r.st));
+    if ((size_t)(sums - sums0) > n_sums && r.rc == 0) { cmgan_set_error("cmgan_tscnet_bwd: statistics scratch exhausted"); r.rc = -1; }
 }
 
 // ---- waveform in, waveform out (evaluation.py:21-53): the launch sequence of signal.enhance / enhance_ragged around forward()
@@ -522,5 +857,98 @@ CMGAN_API int cmgan_enhance(const float* params, const float* wav, long long ldw
     r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
     r.st = (cudaStream_t)stream;
     enhance_walk(r, wav, ldw, B, L, lengths, g, out, ldo);
+    return r.rc;
+}
+
+// ==================================================================================== training: train-mode (or saving eval-mode) forward, backward
+// Workspace of a training call: the saved region (what the backward reads, fixed by the shape), then the scratch of whichever call runs --
+// the forward's or the backward's, which starts with a parameter-gradient stand-in for frozen weights.  Both walks derive the saved layout
+// from the same forward walk, so the backward finds every saved activation where the forward left it.
+struct TrainLayout { size_t keep, fwd, bwd; };
+
+static TrainLayout train_layout(int B, int T, int F, int precision, bool training) {
+    Saved sv;
+    Run f;
+    f.P = nullptr; f.ws = nullptr; f.dry = true; f.precision = precision; f.st = nullptr; f.sv = &sv; f.training = training;
+    forward(f, nullptr, 0, 0, 0, 0, B, T, F, nullptr, nullptr);
+    Run b;
+    b.P = nullptr; b.ws = nullptr; b.dry = true; b.precision = precision; b.st = nullptr; b.training = training;
+    b.alloc((size_t)table().total);
+    backward(b, sv, nullptr, 0, 0, 0, 0, B, T, F, nullptr, nullptr, 0, 0, 0, nullptr);
+    return {(f.ktop + 255) & ~(size_t)255, f.peak, b.peak};
+}
+
+CMGAN_API long long cmgan_tscnet_train_workspace_bytes(int B, int T, int F, int precision) {
+    if (B <= 0 || T <= 0 || F != NFEAT || (precision != 0 && precision != 1)) {
+        cmgan_set_error("cmgan_tscnet_train_workspace_bytes: bad arguments (B=%d T=%d F=%d precision=%d; F must be %d, precision 0 or 1)", B, T, F,
+                        precision, NFEAT);
+        return -1;
+    }
+    if ((long long)B * T * F * CAT >= (1ll << 31)) {
+        cmgan_set_error("cmgan_tscnet_train_workspace_bytes: B * T * F * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); "
+                        "split the batch", CAT, (long long)B * T * F * CAT);
+        return -1;
+    }
+    const TrainLayout L = train_layout(B, T, F, precision, true);      // eval mode keeps the same buffers and needs less statistics scratch
+    return (long long)(L.keep + std::max(L.fwd, L.bwd)) + 256;
+}
+
+// checks shared by both training entries; on success `r` is set up for the walk (saved region at the workspace base, scratch above it)
+static int train_setup(Run& r, Saved& sv, const char* who, const float* params, const float* x, int B, int T, int F, int training,
+                       unsigned long long seed, const unsigned long long* seed_dev, void* workspace, long long workspace_bytes, int precision, void* stream) {
+    CMGAN_REQUIRE(params && x && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE(B > 0 && T > 0 && F == NFEAT, "%s: expected x of shape (B, 2, T, %d), got B=%d T=%d F=%d", who, NFEAT, B, T, F);
+    CMGAN_REQUIRE(precision == 0 || precision == 1, "%s: precision must be 0 (fp32) or 1 (tf32)", who);
+    CMGAN_REQUIRE(training == 0 || training == 1, "%s: training must be 0 (eval) or 1 (train)", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    CMGAN_REQUIRE((long long)B * T * F * CAT < (1ll << 31),
+                  "%s: B * T * F * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split the batch", who, CAT,
+                  (long long)B * T * F * CAT);
+    const long long need = cmgan_tscnet_train_workspace_bytes(B, T, F, precision);
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    const TrainLayout L = train_layout(B, T, F, precision, training == 1);
+    cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
+    r.P = params; r.dry = false; r.precision = precision; r.st = (cudaStream_t)stream;
+    r.sv = &sv; r.kws = static_cast<char*>(workspace);
+    r.ws = r.kws + L.keep; r.cap = (size_t)workspace_bytes - L.keep;
+    r.training = training == 1; r.seed = seed; r.seed_dev = seed_dev;
+    return 0;
+}
+
+CMGAN_API int cmgan_tscnet_fwd_train(float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
+                                     int training, unsigned long long seed, const unsigned long long* seed_dev, float* final_real, float* final_imag,
+                                     void* workspace, long long workspace_bytes, int precision, void* stream) {
+    const char* who = "cmgan_tscnet_fwd_train";
+    CMGAN_REQUIRE(final_real && final_imag, "%s: null pointer", who);
+    Run r;
+    Saved sv;
+    if (train_setup(r, sv, who, params, x, B, T, F, training, seed, seed_dev, workspace, workspace_bytes, precision, stream) != 0) return -1;
+    forward(r, x, sxb, sxc, sxt, sxf, B, T, F, final_real, final_imag);
+    return r.rc;
+}
+
+CMGAN_API int cmgan_tscnet_bwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
+                               int training, unsigned long long seed, const unsigned long long* seed_dev, const float* dfr, const float* dfi, long long sgb,
+                               long long sgt, long long sgf, float* grads, float* dx, void* workspace, long long workspace_bytes, int precision,
+                               void* stream) {
+    const char* who = "cmgan_tscnet_bwd";
+    CMGAN_REQUIRE(grads || dx, "%s: grads and dx are both null: nothing to compute", who);
+    CMGAN_REQUIRE((((uintptr_t)grads) & 15) == 0, "%s: grads must be 16-byte aligned", who);
+    CMGAN_REQUIRE(sgb >= 0 && sgt >= 0 && sgf >= 0, "%s: gradient strides must be non-negative", who);
+    CMGAN_REQUIRE((dfr && dfi) || (long long)(B - 1) * sgb + (long long)(T - 1) * sgt + (long long)(F - 1) * sgf < (long long)B * T * F,
+                  "%s: a null dfr / dfi stands for zeros laid out with the strides of the other; those strides span more than B * T * F elements", who);
+    Run r;
+    Saved sv;
+    if (train_setup(r, sv, who, params, x, B, T, F, training, seed, seed_dev, workspace, workspace_bytes, precision, stream) != 0) return -1;
+    r.quiet = true;          // the forward walk launches nothing here: it only places the saved activations where the forward call left them
+    forward(r, x, sxb, sxc, sxt, sxf, B, T, F, nullptr, nullptr);
+    if (r.rc != 0) return r.rc;
+    r.quiet = false;
+    r.top = r.peak = 0;
+    float* gscratch = r.alloc((size_t)table().total);       // frozen weights: the gradient atomics fused into the data-gradient kernels land here
+    r.G = grads ? grads : gscratch;
+    r.wgrad = grads != nullptr;
+    r.P = params;
+    backward(r, sv, x, sxb, sxc, sxt, sxf, B, T, F, dfr, dfi, sgb, sgt, sgf, dx);
     return r.rc;
 }

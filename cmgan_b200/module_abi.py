@@ -2,7 +2,8 @@
 
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
-out.  torch is used here only to own the device memory."""
+out.  ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
+parameter and input gradients.  torch is used here only to own the device memory."""
 from __future__ import annotations
 
 import ctypes
@@ -92,3 +93,51 @@ def enhance(flat: torch.Tensor, wav: torch.Tensor, lengths=None, cut_len: int = 
     lib().call("cmgan_enhance", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), cut_len,
                out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
     return out
+
+
+def train_workspace_bytes(B: int, T: int, F: int, precision: int) -> int:
+    """workspace of ``cmgan_tscnet_fwd_train`` + ``cmgan_tscnet_bwd`` (one workspace serves the pair; the same size for train and eval mode)"""
+    n = lib().cdll.cmgan_tscnet_train_workspace_bytes(B, T, F, precision)
+    if n < 0:
+        raise RuntimeError(lib().cdll.cmgan_last_error().decode())
+    return n
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def tscnet_forward_train(flat: torch.Tensor, x: torch.Tensor, training: bool, seed: int, seed_dev: torch.Tensor = None, precision: int = 1,
+                         workspace: torch.Tensor = None):
+    """``cmgan_tscnet_fwd_train``: x (B, 2, T, F) on the GPU, any strides -> (final_real, final_imag, workspace).  ``training``: train-mode forward
+    (dropout, BatchNorm batch statistics; the running statistics in ``flat`` are updated in place), else eval mode; either way the activations the
+    backward reads stay in ``workspace``, which the matching ``tscnet_backward`` call takes.  ``seed_dev``: optional device uint64 counter added to
+    every dropout seed (a torch.int64 tensor of one element)."""
+    assert x.is_cuda and flat.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 2
+    B, _, T, F = x.shape
+    if workspace is None:
+        workspace = torch.empty(train_workspace_bytes(B, T, F, precision), dtype=torch.uint8, device=x.device)
+    fr = torch.empty(B, 1, T, F, device=x.device)
+    fi = torch.empty(B, 1, T, F, device=x.device)
+    sb, sc, st, sf = x.stride()
+    lib().call("cmgan_tscnet_fwd_train", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, int(bool(training)), seed & 0xFFFFFFFFFFFFFFFF,
+               _ptr(seed_dev), fr.data_ptr(), fi.data_ptr(), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    return fr, fi, workspace
+
+
+def tscnet_backward(flat: torch.Tensor, x: torch.Tensor, dfr, dfi, grads: torch.Tensor = None, need_dx: bool = True, *, training: bool, seed: int,
+                    seed_dev: torch.Tensor = None, precision: int = 1, workspace: torch.Tensor):
+    """``cmgan_tscnet_bwd`` after ``tscnet_forward_train`` with the same x, flat, training, seed, seed_dev, precision and workspace.
+    dfr / dfi: gradients wrt final_real / final_imag ((B, 1, T, F), or None for zeros).  ``grads``: flat block laid out like ``flat``; the parameter
+    gradients are accumulated into it; None = frozen weights (no weight-gradient GEMM runs).  Returns dx ((B, 2, T, F) contiguous) or None."""
+    assert x.is_cuda and flat.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 2
+    B, _, T, F = x.shape
+    if dfr is not None and dfi is not None and dfr.stride() != dfi.stride():
+        dfr, dfi = dfr.contiguous(), dfi.contiguous()
+    gs = (dfr if dfr is not None else dfi).stride() if (dfr is not None or dfi is not None) else (T * F, T * F, F, 1)
+    dx = torch.empty(B, 2, T, F, device=x.device) if need_dx else None
+    sb, sc, st, sf = x.stride()
+    lib().call("cmgan_tscnet_bwd", flat.data_ptr(), x.data_ptr(), sb, sc, st, sf, B, T, F, int(bool(training)), seed & 0xFFFFFFFFFFFFFFFF,
+               _ptr(seed_dev), _ptr(dfr), _ptr(dfi), gs[0], gs[2], gs[3], _ptr(grads), _ptr(dx), workspace.data_ptr(), workspace.numel(), precision,
+               torch.cuda.current_stream().cuda_stream)
+    return dx

@@ -153,6 +153,29 @@ int cmgan_tscnet_fwd(const float* params, const float* x, long long sxb, long lo
  * encoder's concat buffer is indexed with 32-bit element counts). */
 int cmgan_tscnet_fwd_ragged(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, const int* frames, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
 
+/* ---- module level, training: TSCNet.forward with its activations saved, and TSCNet's backward (parameter and input gradients), one call each.
+ * cmgan_tscnet_fwd_train, training = 1: the train-mode forward (generator.py:160-196 under model.train()).  Dropout p = 0.2 at the five sites of
+ *   every conformer block, with the masks of the counter-based generator (cmgan_dropout_mask) at seed (seed * 1000003 + block * 16 + site + 1)
+ *   mod 2^64 (block = 2 (i - 1) + axis for TSCB_i, site 0..4 = ff1 hidden, ff1 out, attention out, ff2 hidden, ff2 out) plus *seed_dev when
+ *   seed_dev is not null (a device counter: CUDA-graph replays draw fresh masks).  BatchNorm uses batch statistics and updates running_mean /
+ *   running_var in params in place (momentum 0.1, unbiased variance).  num_batches_tracked is not in the block: the caller owns it (at
+ *   momentum 0.1 it affects no value).  training = 0: the eval-mode forward (running statistics, no dropout; params untouched) with the
+ *   activations saved, for input gradients through a frozen eval-mode model.
+ * The workspace (256-byte aligned, >= cmgan_tscnet_train_workspace_bytes(B, T, F, precision), the same for both modes) keeps everything the
+ *   backward reads -- the encoder's concat buffer, raw outputs and normalisation tables, every conformer's input and saved activations, the
+ *   decoders' concat buffers, raw outputs, tables and sub-pixel outputs, the mask tail -- in a region at its start; scratch lies above it.
+ * cmgan_tscnet_bwd: gradients given dfr / dfi (B, 1, T, F) with element strides (sgb, sgt, sgf) (either may be null: zeros, laid out with the
+ *   other's strides, which must then span at most B * T * F elements).  grads: a block laid out like params (cmgan_tscnet_param_info);
+ *   every parameter gradient is ACCUMULATED into it (+=), running-statistic slots are never written.  grads == NULL: frozen weights, no
+ *   weight-gradient GEMM and no head weight gradient runs.  dx: the input gradient, contiguous (B, 2, T, F), or NULL.  Not both NULL.
+ *   Preconditions (not checked on the device): it follows a cmgan_tscnet_fwd_train with the same workspace, B, T, F, training, seed, precision,
+ *   an unchanged *seed_dev, unchanged params (including the running statistics that forward wrote) and an unchanged x; nothing in between
+ *   wrote to the workspace.  Both return -1 (no launch) for null or misaligned pointers (params, grads 16-byte; workspace 256-byte), F != 201,
+ *   B or T <= 0, precision not 0 / 1, training not 0 / 1, a workspace smaller than the query, or B * T * F * 320 >= 2^31. */
+long long cmgan_tscnet_train_workspace_bytes(int B, int T, int F, int precision);
+int cmgan_tscnet_fwd_train(float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, int training, unsigned long long seed, const unsigned long long* seed_dev, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
+int cmgan_tscnet_bwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, int training, unsigned long long seed, const unsigned long long* seed_dev, const float* dfr, const float* dfi, long long sgb, long long sgt, long long sgf, float* grads, float* dx, void* workspace, long long workspace_bytes, int precision, void* stream);
+
 /* ---- module level, waveform in / waveform out: evaluation.py:21-53 (enhance_one_track between load and save) as one call.
  * wav (B, L) fp32 with row stride ldw; out (B, L) fp32 with row stride ldo; neither range may overlap the other.  Per clip: RMS scale,
  * wrap padding to a multiple of 100, the STFT, power compression, TSCNet.forward (params / precision as cmgan_tscnet_fwd), un-compression,
