@@ -16,21 +16,16 @@
 
 #include "common.cuh"
 #include "frontend.cuh"
+#include "module_walk.cuh"
 #include "../../include/cmgan_b200.h"
 
 namespace {
 
+using namespace cmgan_walk;
+
 constexpr int C = 64, CAT = 320, NFEAT = 201;
 
-struct Entry { std::string key; long long off, numel; };
-
-struct Table {
-    std::vector<Entry> e;
-    long long total = 0;
-    void add(const std::string& k, long long n) {
-        e.push_back({k, total, n});
-        total += (n + 3) / 4 * 4;
-    }
+struct Table : ParamTable {
     void norm_prelu(const std::string& p, const char* norm, const char* prelu) {
         add(p + norm + ".weight", C); add(p + norm + ".bias", C); add(p + prelu + ".weight", C);
     }
@@ -90,16 +85,6 @@ const Table& table() {
     static const Table t;
     return t;
 }
-const std::unordered_map<std::string, long long>& offsets() {
-    static const std::unordered_map<std::string, long long> m = [] {
-        std::unordered_map<std::string, long long> o;
-        for (const Entry& e : table().e) o.emplace(e.key, e.off);
-        return o;
-    }();
-    return m;
-}
-
-struct Tabs { float *scale, *shift, *mean, *rstd; int width; };
 
 // ---- what the backward reads, kept by a training forward (cmgan_tscnet_fwd_train) in the saved region of the workspace
 struct FfSaved { float *xn = nullptr, *st = nullptr, *h = nullptr, *a = nullptr; };      // fp32 feed-forward only (tf32 recomputes its hidden layer)
@@ -127,132 +112,11 @@ unsigned drop_thr(bool on) { return on ? (unsigned)std::min(P_DROP * 4294967296.
 float drop_inv(bool on) { return on ? (float)(1.0 / (1.0 - P_DROP)) : 1.f; }
 unsigned long long site_seed(unsigned long long seed, int block_id, int site) { return seed * 1000003ull + (unsigned long long)(block_id * 16 + site + 1); }
 
-template <typename T>
-T* off(T* p, long long n) { return p ? p + n : nullptr; }
-
 // ---- one forward pass = a walk over the launch list; `dry` only sizes the workspace
-struct Run {
-    const float* P;             // parameter block (null in a dry run)
-    char* ws;                   // workspace base (of the scratch region when `sv` is set)
-    size_t top = 0, peak = 0, cap = 0;
-    bool dry;
-    int precision;
-    cudaStream_t st;
-    const int* frames = nullptr;      // ragged batch: valid frames per utterance (device); null = every utterance fills the grid
-    int rc = 0;
-    // training entries only (the inference walks leave these alone)
-    Saved* sv = nullptr;        // forward: keep what the backward reads in the saved region (below the scratch) and record where
-    char* kws = nullptr;        // saved region base
-    size_t ktop = 0;
-    bool quiet = false;         // walk for the addresses only: the backward re-derives the saved layout this way, nothing is launched
-    bool training = false;      // dropout and BatchNorm batch statistics (running statistics updated in place)
-    unsigned long long seed = 0;
-    const unsigned long long* seed_dev = nullptr;
-    float* G = nullptr;         // backward: parameter-gradient block (scratch when the weights are frozen)
-    bool wgrad = true;          // backward: run the weight-gradient GEMMs and the head weight gradient
-
-    long long find(const std::string& key) const {
-        const auto it = offsets().find(key);
-        if (it != offsets().end()) return it->second;
-        cmgan_set_error("cmgan_tscnet: unknown parameter %s", key.c_str());
-        const_cast<Run*>(this)->rc = -1;
-        return -1;
-    }
-    const float* w(const std::string& key) const {
-        if (dry) return nullptr;
-        const long long o = find(key);
-        return o < 0 ? nullptr : P + o;
-    }
-    float* g(const std::string& key) const {
-        if (dry) return nullptr;
-        const long long o = find(key);
-        return o < 0 ? nullptr : G + o;
-    }
-    template <typename T = float>
-    T* alloc(size_t n) {
-        top = (top + 255) & ~(size_t)255;
-        T* p = dry ? nullptr : reinterpret_cast<T*>(ws + top);
-        top += n * sizeof(T);
-        if (top > peak) peak = top;
-        if (!dry && top > cap && rc == 0) { cmgan_set_error("cmgan_tscnet_fwd: workspace too small (%zu bytes needed so far, %zu given)", top, cap); rc = -1; }
-        return p;
-    }
-    // an activation the backward reads: in the saved region when saving, else scratch like any other buffer
-    template <typename T = float>
-    T* keep(size_t n) {
-        if (!sv) return alloc<T>(n);
-        ktop = (ktop + 255) & ~(size_t)255;
-        T* p = dry ? nullptr : reinterpret_cast<T*>(kws + ktop);
-        ktop += n * sizeof(T);
-        return p;
-    }
-    void ok(int r) { if (r != 0 && rc == 0) rc = r; }
-    bool live() const { return !dry && !quiet && rc == 0; }
+struct Run : Walk {
+    Saved* sv = nullptr;        // forward: record where the saved activations are (set together with `saving`)
+    Run() { tab = &table(); tag = "cmgan_tscnet"; who = "cmgan_tscnet_fwd"; }
 };
-
-Tabs make_tabs(Run& r, int G, int width) {
-    Tabs t;
-    t.scale = r.keep((size_t)G * width); t.shift = r.keep((size_t)G * width);
-    t.mean = r.keep((size_t)G * width); t.rstd = r.keep((size_t)G * width);
-    t.width = width;
-    return t;
-}
-
-struct Gemm {
-    CmganGemmArgs a;
-    bool wg = false;
-    Gemm(const float* A, long long lda, const float* W, long long sb_tap, long long sb_k, long long sb_n, const float* bias, float* Cout,
-         long long ldc, long long M, int N, int Cin) {
-        memset(&a, 0, sizeof(a));
-        a.A = A; a.lda = lda; a.B = W; a.sb_tap = sb_tap; a.sb_k = sb_k; a.sb_n = sb_n; a.bias = bias; a.C = Cout; a.ldc = ldc;
-        a.M = (int)M; a.N = N; a.Cin = Cin; a.ntaps = 1;
-        a.mul_y = a.mul_x = a.div_y = a.div_x = 1;
-        a.inv_keep = 1.f; a.pro_inv_keep = 1.f; a.alpha = 1.f; a.pro_alpha = 1.f;
-    }
-    Gemm& conv(int OH, int OW, int IH, int IW, int mul_x = 1, int div_x = 1) {
-        a.conv = 1; a.OH = OH; a.OW = OW; a.IH = IH; a.IW = IW; a.mul_x = mul_x; a.div_x = div_x;
-        return *this;
-    }
-    Gemm& taps(int n, const int* dy, const int* dx) {
-        a.ntaps = n;
-        for (int i = 0; i < n; ++i) { a.dy[i] = dy[i]; a.dx[i] = dx[i]; }
-        return *this;
-    }
-    Gemm& residual(const float* R, long long ldr) { a.epi = CMGAN_EPI_DROP_RES; a.R = R; a.ldr = ldr; return *this; }
-    Gemm& drop(unsigned long long seed, unsigned thr, float inv_keep) { a.seed = seed; a.drop_thr = thr; a.inv_keep = inv_keep; return *this; }
-    Gemm& epi(int e, const float* aux, long long ldaux) { a.epi = e; a.aux = aux; a.ldaux = ldaux; return *this; }
-    // weight gradient: accumulates dW (laid out like W: C = dW, ldc = 0) from A and the upstream gradient rows D
-    Gemm& wgrad(const float* D, long long ldd, float* dbias) { wg = true; a.D = D; a.ldd = ldd; a.dbias = dbias; return *this; }
-    void run(Run& r) {
-        a.precision = r.precision;
-        a.seed_dev = r.seed_dev;
-        if (wg) {
-            if (r.wgrad && r.live()) r.ok(cmgan_gemm_wgrad_f32(&a, r.st));
-            return;
-        }
-        if (r.precision == 1 && a.N % 16 == 0 && a.N <= 256 && a.Cin % 32 == 0) {      // scratch for the re-tiled weight (gemm_args.h)
-            a.ws_floats = (long long)a.N * a.Cin * a.ntaps;
-            a.ws = r.alloc((size_t)a.ws_floats);
-        }
-        if (r.live()) r.ok(cmgan_gemm_rows_f32(&a, r.st));
-    }
-};
-
-// rows_per_t: rows of one frame within a group (row = t * rows_per_t + f); a ragged batch normalises over the valid frames only
-void inst_norm_site(Run& r, const float* x, long long ldx, int G, long long rows, long long rows_per_t, int Cn, const float* gamma, const float* beta,
-                    const Tabs& t, double*& sums) {
-    double* s = sums;
-    sums += (size_t)G * Cn * 2;
-    if (!r.live()) return;
-    if (r.frames) {
-        r.ok(cmgan_norm_stats_ragged(x, ldx, G, rows, Cn, rows_per_t, r.frames, s, r.st));
-        r.ok(cmgan_norm_finalize_ragged(s, rows_per_t, (int)(rows / rows_per_t), r.frames, G, Cn, gamma, beta, t.scale, t.shift, t.mean, t.rstd,
-                                        t.width, r.st));
-        return;
-    }
-    r.ok(cmgan_norm_stats(x, ldx, G, rows, Cn, s, r.st));
-    r.ok(cmgan_norm_finalize(s, rows, G, Cn, 0, gamma, beta, nullptr, nullptr, 0.f, t.scale, t.shift, t.mean, t.rstd, t.width, r.st));
-}
 
 // InstanceNorm2d(affine) + PReLU of a raw (M, 64) tensor, written into dst (generator.py:35-37)
 Tabs norm_prelu_to(Run& r, const float* raw, int G, long long rows, long long rows_per_t, const float* gamma, const float* beta, const float* slope,
@@ -463,17 +327,6 @@ void forward(Run& r, const float* x, long long sxb, long long sxc, long long sxt
 
 // ==================================================================================== backward (network.tscnet_bwd, conformer_block.conformer_bwd)
 // The launch sequence of the Python walk on one stream (ops.WGRAD_STREAM = ops.AUX_STREAM = None, no weight-pack cache, ATTN_BWD_WS off).
-
-// InstanceNorm / BatchNorm (+ PReLU) backward of one site (conformer_block._norm_bwd); `operand`: dx feeds tensor-core contractions
-void norm_bwd(Run& r, const float* x, long long ldx, const float* dact, long long ldd, int G, long long rows, int Cn, int act, int batch_stats,
-              const Tabs& t, const float* slope, float* dx, long long lddx, float* dgamma, float* dbeta, float* dslope, double*& sums, bool operand) {
-    double* s = sums;
-    sums += (size_t)G * Cn * 2;
-    if (!r.live()) return;
-    r.ok(cmgan_norm_bwd_reduce(x, ldx, dact, ldd, G, rows, Cn, act, t.scale, t.shift, t.mean, t.rstd, t.width, slope, s, dslope, r.st));
-    r.ok(cmgan_norm_bwd_apply(x, ldx, dact, ldd, G, rows, Cn, act | (operand && r.precision == 1 ? 16 : 0), batch_stats, t.scale, t.shift, t.mean,
-                              t.rstd, t.width, slope, s, dx, lddx, dgamma, dbeta, r.st));
-}
 
 // LayerNorm backward (+ residual gradients); with dz also the dropout-scaled copy dz = zalpha * mask(zseed) * dx that enters the next branch
 void ln_bwd(Run& r, long long M, const float* dy, const float* x, const float* st, const std::string& name, const float* res, const float* res2,
@@ -869,7 +722,7 @@ struct TrainLayout { size_t keep, fwd, bwd; };
 static TrainLayout train_layout(int B, int T, int F, int precision, bool training) {
     Saved sv;
     Run f;
-    f.P = nullptr; f.ws = nullptr; f.dry = true; f.precision = precision; f.st = nullptr; f.sv = &sv; f.training = training;
+    f.P = nullptr; f.ws = nullptr; f.dry = true; f.precision = precision; f.st = nullptr; f.sv = &sv; f.saving = true; f.training = training;
     forward(f, nullptr, 0, 0, 0, 0, B, T, F, nullptr, nullptr);
     Run b;
     b.P = nullptr; b.ws = nullptr; b.dry = true; b.precision = precision; b.st = nullptr; b.training = training;
@@ -909,7 +762,7 @@ static int train_setup(Run& r, Saved& sv, const char* who, const float* params, 
     const TrainLayout L = train_layout(B, T, F, precision, training == 1);
     cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
     r.P = params; r.dry = false; r.precision = precision; r.st = (cudaStream_t)stream;
-    r.sv = &sv; r.kws = static_cast<char*>(workspace);
+    r.sv = &sv; r.saving = true; r.kws = static_cast<char*>(workspace);
     r.ws = r.kws + L.keep; r.cap = (size_t)workspace_bytes - L.keep;
     r.training = training == 1; r.seed = seed; r.seed_dev = seed_dev;
     return 0;

@@ -3,7 +3,9 @@
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
 out.  ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
-parameter and input gradients.  torch is used here only to own the device memory."""
+parameter and input gradients.  ``cmgan_disc_fwd`` / ``cmgan_disc_bwd`` are the same pair for the metric discriminator (ref: discriminator.py:29-64),
+with the spectral-norm power iteration, parameter gradients through the spectral norm and input gradients.  torch is used here only to own
+the device memory."""
 from __future__ import annotations
 
 import ctypes
@@ -141,3 +143,66 @@ def tscnet_backward(flat: torch.Tensor, x: torch.Tensor, dfr, dfi, grads: torch.
                _ptr(seed_dev), _ptr(dfr), _ptr(dfi), gs[0], gs[2], gs[3], _ptr(grads), _ptr(dx), workspace.data_ptr(), workspace.numel(), precision,
                torch.cuda.current_stream().cuda_stream)
     return dx
+
+
+# ---- the metric discriminator (ndf = 16): cmgan_disc_fwd / cmgan_disc_bwd
+def disc_param_table() -> List[Tuple[str, int, int]]:
+    """[(state_dict key, offset in floats, element count)] of the discriminator's flat block, in state_dict order (u / v buffers included)"""
+    L = lib().cdll
+    out = []
+    key, off, n = ctypes.c_char_p(), ctypes.c_longlong(), ctypes.c_longlong()
+    for i in range(L.cmgan_disc_param_count()):
+        lib().call("cmgan_disc_param_info", i, ctypes.byref(key), ctypes.byref(off), ctypes.byref(n))
+        out.append((key.value.decode(), off.value, n.value))
+    return out
+
+
+def pack_disc_params(state_dict: Dict[str, torch.Tensor], device) -> torch.Tensor:
+    """Discriminator(16) state_dict (reference key names) -> the flat fp32 block ``cmgan_disc_fwd`` reads"""
+    flat = torch.zeros(lib().cdll.cmgan_disc_param_floats(), dtype=torch.float32, device=device)
+    for key, off, n in disc_param_table():
+        t = state_dict[key]
+        assert t.numel() == n, f"{key}: {t.numel()} elements, the C table expects {n}"
+        flat[off:off + n].copy_(t.detach().reshape(-1).to(torch.float32))
+    return flat
+
+
+def disc_workspace_bytes(B: int, H: int, W: int, precision: int) -> int:
+    """workspace of one ``cmgan_disc_fwd`` + ``cmgan_disc_bwd`` pair (the same size for train and eval mode)"""
+    n = lib().cdll.cmgan_disc_workspace_bytes(B, H, W, precision)
+    if n < 0:
+        raise RuntimeError(lib().cdll.cmgan_last_error().decode())
+    return n
+
+
+def disc_forward(flat: torch.Tensor, x: torch.Tensor, y: torch.Tensor, training: bool, seed: int, seed_dev: torch.Tensor = None, precision: int = 1,
+                 workspace: torch.Tensor = None):
+    """``cmgan_disc_fwd``: x, y (B, 1, H, W) on the GPU, any strides (y may be x) -> (out (B, 1), workspace).  ``training``: one power iteration
+    per spectrally normalised weight (weight_u / weight_v in ``flat`` updated in place) and dropout, else eval mode.  Either way the activations
+    the backward reads stay in ``workspace``, which the matching ``disc_backward`` takes; each outstanding forward needs its own."""
+    assert x.is_cuda and y.is_cuda and flat.is_cuda and x.dtype == torch.float32 and y.dtype == torch.float32
+    assert x.dim() == 4 and x.shape[1] == 1 and y.shape == x.shape
+    B, _, H, W = x.shape
+    if workspace is None:
+        workspace = torch.empty(disc_workspace_bytes(B, H, W, precision), dtype=torch.uint8, device=x.device)
+    out = torch.empty(B, 1, device=x.device)
+    sx, sy = x.stride(), y.stride()
+    lib().call("cmgan_disc_fwd", flat.data_ptr(), x.data_ptr(), sx[0], sx[2], sx[3], y.data_ptr(), sy[0], sy[2], sy[3], B, H, W, int(bool(training)),
+               seed & 0xFFFFFFFFFFFFFFFF, _ptr(seed_dev), out.data_ptr(), workspace.data_ptr(), workspace.numel(), precision,
+               torch.cuda.current_stream().cuda_stream)
+    return out, workspace
+
+
+def disc_backward(flat: torch.Tensor, dout: torch.Tensor, shape, grads: torch.Tensor = None, need_dx: bool = True, need_dy: bool = True, *,
+                  training: bool, seed: int, seed_dev: torch.Tensor = None, precision: int = 1, workspace: torch.Tensor):
+    """``cmgan_disc_bwd`` after ``disc_forward`` with the same shape ((B, 1, H, W), e.g. x.shape), training, seed, seed_dev, precision and
+    workspace.  dout: gradient wrt out (B, 1).  ``grads``: flat block laid out like ``flat``; the parameter gradients are accumulated into it;
+    None = frozen weights (no weight-gradient GEMM, no spectral-norm backward).  Returns (dx, dy), each (B, 1, H, W) contiguous or None."""
+    B, _, H, W = shape
+    dout = dout.contiguous()
+    assert dout.is_cuda and dout.numel() == B
+    dx = torch.empty(B, 1, H, W, device=dout.device) if need_dx else None
+    dy = torch.empty(B, 1, H, W, device=dout.device) if need_dy else None
+    lib().call("cmgan_disc_bwd", flat.data_ptr(), B, H, W, int(bool(training)), seed & 0xFFFFFFFFFFFFFFFF, _ptr(seed_dev), dout.data_ptr(), _ptr(grads),
+               _ptr(dx), _ptr(dy), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    return dx, dy

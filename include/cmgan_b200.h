@@ -176,6 +176,34 @@ long long cmgan_tscnet_train_workspace_bytes(int B, int T, int F, int precision)
 int cmgan_tscnet_fwd_train(float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, int training, unsigned long long seed, const unsigned long long* seed_dev, float* final_real, float* final_imag, void* workspace, long long workspace_bytes, int precision, void* stream);
 int cmgan_tscnet_bwd(const float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F, int training, unsigned long long seed, const unsigned long long* seed_dev, const float* dfr, const float* dfi, long long sgb, long long sgt, long long sgf, float* grads, float* dx, void* workspace, long long workspace_bytes, int precision, void* stream);
 
+/* ---- module level, training: the metric discriminator (discriminator.py:29-64, ndf = 16 as train.py:55) forward with its activations saved, and
+ * its backward (parameter gradients through the spectral norm, input gradients), one call each.
+ * params = the 34 floating-point state_dict tensors of the reference Discriminator(16) in state_dict order, the spectral-norm triplets
+ *   weight_orig / weight_u / weight_v included, each starting at a multiple of 4 floats (cmgan_disc_param_info enumerates key / offset / numel).
+ * cmgan_disc_fwd: x, y are (B, 1, H, W) magnitudes with element strides (the trainer passes (B, 1, F, T) permuted views of (B, 1, T, F)
+ *   buffers; x == y is allowed); out is (B, 1).  H, W >= 16.  training = 1: one power iteration per spectrally normalised weight, weight_u /
+ *   weight_v updated in place in params (as torch's spectral_norm in train mode); Dropout(0.3) with the mask of the counter-based generator
+ *   (cmgan_dropout_mask) at seed, plus *seed_dev when seed_dev is not null.  training = 0: stored u / v, no dropout, params untouched; the
+ *   activations are still saved, so a frozen eval-mode discriminator can be differentiated.
+ * The workspace (256-byte aligned, >= cmgan_disc_workspace_bytes(B, H, W, precision), the same for both modes) keeps everything the backward
+ *   reads -- the stacked input, every layer's input, raw output and InstanceNorm tables, W / sigma, sigma and the [u | v] THIS forward used for
+ *   all six spectrally normalised weights, the pooled features and their arg-max, both linear layers' outputs and out -- in a region at its
+ *   start.  Each forward whose backward is still to come needs its own workspace: a later train-mode forward iterates u / v in params again.
+ * cmgan_disc_bwd: dout (B, 1) contiguous.  grads: a block laid out like params; every parameter gradient is ACCUMULATED into it (+=), the
+ *   weight_u / weight_v slots are never written.  grads == NULL: frozen weights, no weight-gradient GEMM and no spectral-norm backward runs.
+ *   dx, dy: the input gradients, contiguous (B, 1, H, W), either may be NULL; not all three NULL.  Preconditions (not checked on the device): it
+ *   follows a cmgan_disc_fwd with the same workspace, B, H, W, training, seed, precision and an unchanged *seed_dev; the non-buffer parameters
+ *   are unchanged; nothing in between wrote to the workspace.  The backward reads nothing else: x, y, weight_u and weight_v may have changed.
+ * precision 0 = exact fp32, 1 = tf32 tensor cores for the convolutions (the two linear layers always run exact fp32).  Both return -1 (no
+ *   launch) for null or misaligned pointers (params, grads 16-byte; workspace 256-byte), B <= 0, H or W < 16, precision not 0 / 1, training
+ *   not 0 / 1, a workspace smaller than the query, or B * H * W > 2^31 - 128 (the GEMMs count rows in 32 bits). */
+int cmgan_disc_param_count(void);
+long long cmgan_disc_param_floats(void);
+int cmgan_disc_param_info(int index, const char** key, long long* offset, long long* numel);
+long long cmgan_disc_workspace_bytes(int B, int H, int W, int precision);
+int cmgan_disc_fwd(float* params, const float* x, long long sxb, long long sxh, long long sxw, const float* y, long long syb, long long syh, long long syw, int B, int H, int W, int training, unsigned long long seed, const unsigned long long* seed_dev, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
+int cmgan_disc_bwd(const float* params, int B, int H, int W, int training, unsigned long long seed, const unsigned long long* seed_dev, const float* dout, float* grads, float* dx, float* dy, void* workspace, long long workspace_bytes, int precision, void* stream);
+
 /* ---- module level, waveform in / waveform out: evaluation.py:21-53 (enhance_one_track between load and save) as one call.
  * wav (B, L) fp32 with row stride ldw; out (B, L) fp32 with row stride ldo; neither range may overlap the other.  Per clip: RMS scale,
  * wrap padding to a multiple of 100, the STFT, power compression, TSCNet.forward (params / precision as cmgan_tscnet_fwd), un-compression,
