@@ -451,7 +451,7 @@ __global__ void recombine_kernel(const float* __restrict__ m1, MaskTail mt, cons
 }
 
 // backward: dfr, dfi with strides (gb, gt, gf) -> dcplx (M, 2), dz (M) = grad wrt the IN(1)+PReLU(1) output;
-// dslope_f (F), dfcw, dfcb accumulated
+// dslope_f (F), dfcw, dfcb accumulated.  At z2 = 0 the slope branch, as torch's PReLU backward.
 __global__ void recombine_bwd_kernel(const float* __restrict__ m1, MaskTail mt, const float* __restrict__ x, long sb, long sc, long st, long sf,
                                      const float* __restrict__ dfr, const float* __restrict__ dfi, long gb, long gt, long gf, int T, int F,
                                      long M, float* __restrict__ dcplx, float* __restrict__ dz, float* __restrict__ dslope_f,
@@ -470,7 +470,7 @@ __global__ void recombine_bwd_kernel(const float* __restrict__ m1, MaskTail mt, 
         reinterpret_cast<float2*>(dcplx)[m] = make_float2(gr, gi);
         float dmask = gr * re + gi * im;
         float dz2 = dmask;
-        if (z2 < 0.f) { dz2 = dmask * __ldg(mt.slope_f + f); atomicAdd(dslope_f + f, dmask * z2); }
+        if (!(z2 > 0.f)) { dz2 = dmask * __ldg(mt.slope_f + f); atomicAdd(dslope_f + f, dmask * z2); }
         pw = dz2 * z; pb = dz2;
         dz[m] = dz2 * mt.fcw[0];
     }

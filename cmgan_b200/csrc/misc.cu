@@ -169,7 +169,8 @@ __global__ void __launch_bounds__(1024) spectral_norm_bwd_kernel(const float* __
     }
 }
 
-// out[b, c] = max over rows of prelu(x*scale+shift);  arg[b, c] = row index (within the group) of the max
+// out[b, c] = max over rows of prelu(x*scale+shift);  arg[b, c] = row index (within the group) of the max: the first of tied rows, and
+// as in torch's adaptive_max_pool2d a NaN wins (the last NaN of the window), so the output is NaN and its gradient goes to that row
 __global__ void norm_maxpool_kernel(const float* __restrict__ x, long rows, int C, const float* __restrict__ scale, const float* __restrict__ shift,
                                     const float* __restrict__ slope, float* __restrict__ out, int* __restrict__ arg) {
     int b = blockIdx.x, c = threadIdx.x;
@@ -179,7 +180,7 @@ __global__ void norm_maxpool_kernel(const float* __restrict__ x, long rows, int 
     for (long r = 0; r < rows; ++r) {
         float z = __ldg(x + ((long)b * rows + r) * C + c) * sc + sh;
         if (z < 0.f) z *= a;
-        if (z > best) { best = z; bi = (int)r; }
+        if (z > best || isnan(z)) { best = z; bi = (int)r; }
     }
     out[b * C + c] = best;
     if (arg) arg[b * C + c] = bi;
@@ -192,7 +193,8 @@ __global__ void maxpool_bwd_kernel(const float* __restrict__ dout, const int* __
     dact[i] = (arg[b * C + c] == (int)r) ? dout[b * C + c] : 0.f;
 }
 
-// y = prelu(x * drop(i), slope[c])   (Dropout(0.3) then PReLU(64), discriminator.py:55-56); in place allowed
+// y = prelu(x * drop(i), slope[c])   (Dropout(0.3) then PReLU(64), discriminator.py:55-56); in place allowed.  The backward takes the slope
+// branch at z = 0, as torch's PReLU backward does.
 __global__ void drop_prelu_kernel(const float* __restrict__ x, long n, int C, const float* __restrict__ slope, unsigned long long seed,
                                   unsigned thr, float inv_keep, float* __restrict__ y, const unsigned long long* __restrict__ seed_dev) {
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -210,7 +212,7 @@ __global__ void drop_prelu_bwd_kernel(const float* __restrict__ x, const float* 
     float ds = cmgan_drop_scale(seed, (uint64_t)i, thr, inv_keep);
     float z = x[i] * ds;
     float g = dy[i];
-    if (z < 0.f) { atomicAdd(dslope + (i % C), g * z); g *= slope[i % C]; }
+    if (!(z > 0.f)) { atomicAdd(dslope + (i % C), g * z); g *= slope[i % C]; }
     dx[i] = g * ds;
 }
 // y = sigmoid(slope * x)  (LearnableSigmoid(1), utils.py:42-50)

@@ -145,6 +145,16 @@ __device__ __forceinline__ long stats_rows(long rows_per_group, long rows_per_t,
     return (long)clamp_len(__ldg(tlen + grp), (int)(rows_per_group / rows_per_t)) * rows_per_t;
 }
 
+// The threads accumulate x - p in float, p = the group's row 0 (per channel, the same in every block of the group): with a large mean
+// (mean / std = 100) raw float sums of x and x^2 lose the variance to cancellation in E[x^2] - E[x]^2, centred ones do not.  The block
+// partials (s' = sum (x - p), q' = sum (x - p)^2 over its n rows) go back to raw sums in double, so the sums layout, cmgan_norm_finalize
+// and every other producer of the sums (the depthwise conv's BatchNorm sums) stay as they are.
+__device__ __forceinline__ void pivot_sums(double s, double q, float p, long n, double* __restrict__ dst) {
+    const double pd = p;
+    atomicAdd(dst, s + (double)n * pd);
+    atomicAdd(dst + 1, q + 2.0 * pd * s + (double)n * pd * pd);
+}
+
 template <bool RAGGED>
 __global__ void norm_stats_kernel(const float* __restrict__ x, long ldx, long rows_per_group, int C, int chunk,
                                   double* __restrict__ sums, const int* __restrict__ tlen, long rows_per_t) {
@@ -157,15 +167,15 @@ __global__ void norm_stats_kernel(const float* __restrict__ x, long ldx, long ro
     int c = threadIdx.x % C, rg = threadIdx.x / C, nrg = blockDim.x / C;
     float s = 0.f, q = 0.f;
     const float* base = x + ((long)grp * rows_per_group) * ldx + c;
+    const float p = __ldg(base);                    // pivot: row 0 of the group (see pivot_sums)
     if (rg < nrg)
-        for (long r = r_beg + rg; r < r_end; r += nrg) { float v = __ldg(base + r * ldx); s += v; q = fmaf(v, v, q); }
+        for (long r = r_beg + rg; r < r_end; r += nrg) { float v = __ldg(base + r * ldx) - p; s += v; q = fmaf(v, v, q); }
     sm[threadIdx.x * 2] = s; sm[threadIdx.x * 2 + 1] = q;
     __syncthreads();
     if (threadIdx.x < C) {
         double ds = 0.0, dq = 0.0;
         for (int g = 0; g < nrg; ++g) { ds += sm[(g * C + c) * 2]; dq += sm[(g * C + c) * 2 + 1]; }
-        atomicAdd(sums + ((long)grp * C + c) * 2, ds);
-        atomicAdd(sums + ((long)grp * C + c) * 2 + 1, dq);
+        pivot_sums(ds, dq, p, r_end - r_beg, sums + ((long)grp * C + c) * 2);
     }
 }
 
@@ -182,10 +192,12 @@ __global__ void norm_stats4_kernel(const float* __restrict__ x, long ldx, long r
     const int c4 = threadIdx.x % cv, rg = threadIdx.x / cv, nrg = blockDim.x / cv;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
     const float* base = x + ((long)grp * rows_per_group) * ldx + c4 * 4;
+    const float4 p = __ldg(reinterpret_cast<const float4*>(base));      // pivot: row 0 of the group (see pivot_sums)
     if (rg < nrg) {
 #pragma unroll 4
         for (long r = r_beg + rg; r < r_end; r += nrg) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(base + r * ldx));
+            float4 v = __ldg(reinterpret_cast<const float4*>(base + r * ldx));
+            v.x -= p.x; v.y -= p.y; v.z -= p.z; v.w -= p.w;
             s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
             q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
         }
@@ -197,8 +209,7 @@ __global__ void norm_stats4_kernel(const float* __restrict__ x, long ldx, long r
         const int c = threadIdx.x, cc = c >> 2, j = c & 3;
         double ds = 0.0, dq = 0.0;
         for (int g = 0; g < nrg; ++g) { ds += sm[g * cv + cc][j]; dq += sm[g * cv + cc][4 + j]; }
-        atomicAdd(sums + ((long)grp * C + c) * 2, ds);
-        atomicAdd(sums + ((long)grp * C + c) * 2 + 1, dq);
+        pivot_sums(ds, dq, __ldg(x + ((long)grp * rows_per_group) * ldx + c), r_end - r_beg, sums + ((long)grp * C + c) * 2);
     }
 }
 
@@ -239,7 +250,8 @@ __global__ void norm_finalize_kernel(const double* __restrict__ sums, long n, in
 }
 
 // backward pass 1.  z = x*scale + shift; act: 0 none, 1 PReLU(slope[c]);  g = dact * act'(z)
-//   S[(grp*C+c)*2 + {0,1}] += sum g, sum g*xhat   (xhat = (x - mean) * rstd);   dslope[c] += sum dact * z * [z<0]
+//   S[(grp*C+c)*2 + {0,1}] += sum g, sum g*xhat   (xhat = (x - mean) * rstd);   dslope[c] += sum dact * z * [z<=0]
+//   (at z = 0 the slope branch, as torch's PReLU backward: dx = slope * dact there)
 __global__ void norm_bwd_reduce_kernel(const float* __restrict__ x, long ldx, const float* __restrict__ dact, long ldd,
                                        long rows_per_group, int C, int chunk, int act, const float* __restrict__ scale,
                                        const float* __restrict__ shift, const float* __restrict__ mean,
@@ -261,7 +273,7 @@ __global__ void norm_bwd_reduce_kernel(const float* __restrict__ x, long ldx, co
             float d = __ldg(dact + (rb + r) * ldd + c);
             float z = v * sc + sh;
             float gq = d;
-            if (act && z < 0.f) { gq = d * a; s3 = fmaf(d, z, s3); }
+            if (act && !(z > 0.f)) { gq = d * a; s3 = fmaf(d, z, s3); }
             s1 += gq; s2 = fmaf(gq, (v - mu) * rs, s2);
         }
     }
@@ -306,7 +318,7 @@ __global__ void norm_bwd_reduce4_kernel(const float* __restrict__ x, long ldx, c
             for (int j = 0; j < 4; ++j) {
                 const float z = fmaf(v[j], sc[j], sh[j]);
                 float gq = d[j];
-                if (act && z < 0.f) { gq = d[j] * a[j]; s3[j] = fmaf(d[j], z, s3[j]); }
+                if (act && !(z > 0.f)) { gq = d[j] * a[j]; s3[j] = fmaf(d[j], z, s3[j]); }
                 s1[j] += gq; s2[j] = fmaf(gq, (v[j] - mu[j]) * rs[j], s2[j]);
             }
         }
@@ -349,7 +361,7 @@ __global__ void norm_bwd_apply_kernel(const float* __restrict__ x, long ldx, con
     for (long r = r_beg + rg; r < r_end; r += nrg) {
         const float v = __ldg(x + (rb + r) * ldx + c), d = __ldg(dact + (rb + r) * ldd + c);
         const float z = v * sc + sh;
-        const float gq = (act && z < 0.f) ? d * a : d;
+        const float gq = (act && !(z > 0.f)) ? d * a : d;
         dx[(rb + r) * lddx + c] = cmgan_maybe_rna(sc * (gq - m1 - (v - mu) * rs * m2), rnd);
     }
 }
@@ -392,7 +404,7 @@ __global__ void norm_bwd_apply4_kernel(const float* __restrict__ x, long ldx, co
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const float z = fmaf(v[j], sc[j], sh[j]);
-            const float gq = (act && z < 0.f) ? d[j] * a[j] : d[j];
+            const float gq = (act && !(z > 0.f)) ? d[j] * a[j] : d[j];
             o[j] = cmgan_maybe_rna(sc[j] * (gq - m1[j] - (v[j] - mu[j]) * rs[j] * m2[j]), rnd);
         }
         *reinterpret_cast<float4*>(dx + (rb + r) * lddx + c4 * 4) = make_float4(o[0], o[1], o[2], o[3]);

@@ -200,8 +200,27 @@ def test_layernorm_bwd_dropout_scaled_copy():
     _chk(dz, (alpha * dx1).double(), 1e-6, "ln_bwd_drop dz (no dropout)")
 
 
-@pytest.mark.parametrize("Cn,G,rows,act", [(64, 2, 777, 1), (1, 3, 500, 1), (128, 1, 900, 0), (16, 2, 300, 1)])
-def test_group_norm_fwd_bwd(Cn, G, rows, act):
+def _rows_on(t, ld, off, fill=float("nan")):
+    """(rows, C) -> a device buffer holding the rows at leading dimension ``ld``, starting ``off`` floats past the (aligned) base; the padding
+    columns hold ``fill``.  Returns (buffer, (rows, ld) view at the offset)."""
+    n, c = t.shape
+    b = torch.full((off + n * ld,), fill, device=DEV)
+    v = b[off:].view(n, ld)
+    v[:, :c] = t.to(DEV)
+    return b, v
+
+
+# layout "aligned": contiguous, 16-byte aligned rows (the 128-bit kernels wherever C % 4 == 0); "padded": leading dimension C + 1, and
+# "offset": the base one float past an aligned address -- both take the scalar kernels
+@pytest.mark.parametrize("Cn,G,rows,act,layout", [
+    pytest.param(64, 2, 777, 1, "aligned", id="64-2-777-1"), pytest.param(1, 3, 500, 1, "aligned", id="1-3-500-1"),
+    pytest.param(128, 1, 900, 0, "aligned", id="128-1-900-0"), pytest.param(16, 2, 300, 1, "aligned", id="16-2-300-1"),
+    pytest.param(256, 2, 300, 1, "aligned", id="256-2-300-1-aligned"), pytest.param(2, 2, 301, 1, "offset", id="2-2-301-1-offset"),
+    pytest.param(64, 2, 777, 1, "padded", id="64-2-777-1-padded"), pytest.param(64, 3, 500, 1, "offset", id="64-3-500-1-offset"),
+    pytest.param(256, 1, 333, 1, "padded", id="256-1-333-1-padded")])
+def test_group_norm_fwd_bwd(Cn, G, rows, act, layout):
+    ld = Cn + 1 if layout == "padded" else Cn
+    off = 1 if layout == "offset" else 0
     x = (_rand(G * rows, Cn, seed=40) * 2.0 + 0.7).double().requires_grad_(True)
     g = (_rand(Cn, seed=41) + 1.5).double().requires_grad_(True)
     b = _rand(Cn, seed=42).double().requires_grad_(True)
@@ -213,27 +232,102 @@ def test_group_norm_fwd_bwd(Cn, G, rows, act):
     y = torch.where(z >= 0, z, z * a) if act else z
     dy = _rand(G, rows, Cn, seed=44)
     y.backward(dy.double())
-    xd = x.detach().float().to(DEV)
+    xb, _ = _rows_on(x.detach().float(), ld, off)
+    xd = (xb, off)
     sums = torch.zeros(G * Cn * 2, dtype=torch.float64, device=DEV)
-    call("cmgan_norm_stats", xd, Cn, G, rows, Cn, sums)
+    call("cmgan_norm_stats", xd, ld, G, rows, Cn, sums)
     sc, sh, mu, rs = (torch.empty(G, Cn, device=DEV) for _ in range(4))
     gd, bd, ad = g.detach().float().to(DEV), b.detach().float().to(DEV), a.detach().float().to(DEV)
     call("cmgan_norm_finalize", sums, rows, G, Cn, 0, gd, bd, None, None, 0.0, sc, sh, mu, rs, Cn)
-    yd = torch.empty(G * rows, Cn, device=DEV)
-    call("cmgan_norm_apply", xd, Cn, G, rows, Cn, act, sc, sh, Cn, ad, yd, Cn)
-    _chk(yd.view(G, rows, Cn), y, 5e-6, f"norm apply C={Cn}")
+    yb, yv = _rows_on(torch.full((G * rows, Cn), float("nan")), ld, off, fill=-3.0)
+    call("cmgan_norm_apply", xd, ld, G, rows, Cn, act, sc, sh, Cn, ad, (yb, off), ld)
+    _chk(yv[:, :Cn].reshape(G, rows, Cn), y, 5e-6, f"norm apply C={Cn} {layout}")
+    assert (yv[:, Cn:] == -3.0).all()
     S = torch.zeros(G * Cn * 2, dtype=torch.float64, device=DEV)
     dsl = torch.zeros(Cn, device=DEV)
-    dyd = dy.view(-1, Cn).to(DEV)
-    call("cmgan_norm_bwd_reduce", xd, Cn, dyd, Cn, G, rows, Cn, act, sc, sh, mu, rs, Cn, ad, S, dsl)
-    dx = torch.empty(G * rows, Cn, device=DEV)
+    dyb, _ = _rows_on(dy.view(-1, Cn), ld, off)
+    dyd = (dyb, off)
+    call("cmgan_norm_bwd_reduce", xd, ld, dyd, ld, G, rows, Cn, act, sc, sh, mu, rs, Cn, ad, S, dsl)
+    dxb, dxv = _rows_on(torch.full((G * rows, Cn), float("nan")), ld, off, fill=-3.0)
     dg, db = torch.zeros(Cn, device=DEV), torch.zeros(Cn, device=DEV)
-    call("cmgan_norm_bwd_apply", xd, Cn, dyd, Cn, G, rows, Cn, act, 1, sc, sh, mu, rs, Cn, ad, S, dx, Cn, dg, db)
+    call("cmgan_norm_bwd_apply", xd, ld, dyd, ld, G, rows, Cn, act, 1, sc, sh, mu, rs, Cn, ad, S, (dxb, off), ld, dg, db)
+    dx = dxv[:, :Cn]
+    assert (dxv[:, Cn:] == -3.0).all()
     _chk(dx, x.grad, 1e-5, "norm bwd dx")
     _chk(dg, g.grad, 1e-5, "norm bwd dgamma")
     _chk(db, b.grad, 1e-5, "norm bwd dbeta")
     if act:
         _chk(dsl, a.grad, 1e-5, "norm bwd dslope")
+
+
+@pytest.mark.parametrize("n", [1, 2, 777])
+def test_norm_finalize_running_statistics(n):
+    """train-mode BatchNorm1d (mode 0 with running statistics: momentum, unbiased variance) and eval-mode BatchNorm1d (mode 1: the
+    tables from the running statistics) against F.batch_norm in float64.  With one row torch refuses to train; the kernel then keeps the
+    biased variance (0) in the running update, formed here by hand."""
+    C, mom = 128, 0.1
+    x = _rand(n, C, seed=80) * 1.5 + 0.3
+    g, b = _rand(C, seed=81) + 1.5, _rand(C, seed=82)
+    rm0, rv0 = _rand(C, seed=83), _rand(C, seed=84).abs() + 0.5
+    xd, gd, bd = x.to(DEV), g.to(DEV), b.to(DEV)
+    rm, rv = rm0.clone().to(DEV), rv0.clone().to(DEV)
+    sums = torch.zeros(C * 2, dtype=torch.float64, device=DEV)
+    call("cmgan_norm_stats", xd, C, 1, n, C, sums)
+    sc, sh, mu, rs = (torch.full((C,), float("nan"), device=DEV) for _ in range(4))
+    call("cmgan_norm_finalize", sums, n, 1, C, 0, gd, bd, rm, rv, mom, sc, sh, mu, rs, C)
+    rm64, rv64 = rm0.double().clone(), rv0.double().clone()
+    if n > 1:
+        y64 = F.batch_norm(x.double(), rm64, rv64, g.double(), b.double(), training=True, momentum=mom, eps=1e-5)
+    else:
+        rm64 = (1 - mom) * rm64 + mom * x.double()[0]
+        rv64 = (1 - mom) * rv64
+        y64 = b.double().expand(1, C)
+    _chk(rm, rm64, 1e-6, f"running mean n={n}")
+    _chk(rv, rv64, 1e-6, f"running var n={n}")
+    y = torch.empty(n, C, device=DEV)
+    call("cmgan_norm_apply", xd, C, 1, n, C, 0, sc, sh, C, None, y, C)
+    if n > 1:
+        _chk(y, y64, 5e-6, f"train-mode BatchNorm n={n}")
+    else:       # variance 0: scale = gamma / sqrt(eps), so y = x scale + (beta - mean scale) cancels two terms of size |x gamma| / sqrt(eps)
+        terms = 2 * x.double().abs() * g.double().abs() / math.sqrt(1e-5) + b.double().abs()
+        err = (y.cpu().double() - y64).abs()
+        assert (err <= 4 * 2.0 ** -24 * terms).all(), f"train-mode BatchNorm n=1: max-abs err {err.max().item():.3e}"
+    # mode 1 reads the running statistics and leaves them unchanged
+    rm_now, rv_now = rm.clone(), rv.clone()
+    call("cmgan_norm_finalize", None, n, 1, C, 1, gd, bd, rm, rv, mom, sc, sh, mu, rs, C)
+    assert torch.equal(rm, rm_now) and torch.equal(rv, rv_now)
+    assert torch.equal(mu, rm_now)
+    _chk(rs, 1.0 / torch.sqrt(rv_now.double().cpu() + 1e-5), 1e-6, "eval-mode rstd")
+    call("cmgan_norm_apply", xd, C, 1, n, C, 0, sc, sh, C, None, y, C)
+    ref = F.batch_norm(x.double(), rm_now.double().cpu(), rv_now.double().cpu(), g.double(), b.double(), training=False, eps=1e-5)
+    _chk(y, ref, 5e-6, f"eval-mode BatchNorm n={n}")
+
+
+@pytest.mark.parametrize("offset", [10.0, 100.0])
+@pytest.mark.parametrize("layout", ["aligned", "padded"])
+def test_norm_stats_dc_offset(offset, layout):
+    """InstanceNorm of x = offset + N(0, 1), 20200 rows x 64 channels: the normalised output within 4x the error of torch's float32
+    F.instance_norm against float64 on the same input.  Raw float sums of x and x^2 lose the variance to cancellation at mean / std = 100;
+    the statistics kernels sum x - (the group's first row) instead."""
+    G, rows, C = 1, 20200, 64
+    ld = C + 1 if layout == "padded" else C
+    x = _rand(G * rows, C, seed=90) + offset
+    x64 = x.double().view(G, rows, C).permute(0, 2, 1)
+    ref = F.instance_norm(x64, eps=1e-5)
+    err_torch = (F.instance_norm(x.view(G, rows, C).permute(0, 2, 1).contiguous(), eps=1e-5).double() - ref).abs().max().item()
+    xb, _ = _rows_on(x, ld, 0)
+    sums = torch.zeros(G * C * 2, dtype=torch.float64, device=DEV)
+    call("cmgan_norm_stats", xb, ld, G, rows, C, sums)
+    sc, sh, mu, rs = (torch.empty(G, C, device=DEV) for _ in range(4))
+    ones, zeros = torch.ones(C, device=DEV), torch.zeros(C, device=DEV)
+    call("cmgan_norm_finalize", sums, rows, G, C, 0, ones, zeros, None, None, 0.0, sc, sh, mu, rs, C)
+    y = torch.empty(G * rows, C, device=DEV)
+    call("cmgan_norm_apply", xb, ld, G, rows, C, 0, sc, sh, C, None, y, C)
+    err = (y.cpu().double().view(G, rows, C).permute(0, 2, 1) - ref).abs().max().item()
+    rstd64 = 1.0 / torch.sqrt(x64.var(2, unbiased=False) + 1e-5)
+    rstd_err = ((rs.cpu().double() - rstd64).abs() / rstd64).max().item()
+    print(f"[parity] DC offset {offset} ({layout}): rstd rel err {rstd_err:.3e}, output max-abs {err:.3e}, torch fp32 instance_norm {err_torch:.3e}")
+    assert err <= 4 * err_torch, f"normalised output error {err:.3e} > 4 x torch's {err_torch:.3e} (rstd rel err {rstd_err:.3e})"
 
 
 # ------------------------------------------------------------------------------------------------ attention
