@@ -79,7 +79,11 @@ __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __r
 #pragma unroll
     for (int k = 0; k < KS; ++k) wr[k] = __ldg(w + c * KS + k);
     const float bs = __ldg(bias + c);
-    float s1 = 0.f, s2 = 0.f;
+    // BatchNorm partials of the thread's outputs, centred on p = the first accumulator of its first tile (as norm_stats centres on a
+    // group's first row): the output sits near bias + conv(mean u), and raw float sums of y and y^2 at mean / std = 100 lose the
+    // variance to cancellation; cnt counts the outputs summed
+    float s1 = 0.f, s2 = 0.f, piv = 0.f;
+    int cnt = 0;
     int L = sg.L, tps = (sg.L + CK - 1) / CK;
     long total = (long)sg.n_seq * tps;
     if (RAGGED) {
@@ -132,13 +136,20 @@ __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __r
                 for (int i = 0; i < TOK; ++i)
                     if (m - i >= 0 && m - i < KS) acc[i] = fmaf(wr[m - i], u, acc[i]);
             }
+            if (!RAGGED) {
+                if (cnt == 0) piv = acc[0];                     // any value near the outputs centres them; one per thread
+                cnt += max(0, min(TOK, L - tok0));
+            }
 #pragma unroll
             for (int i = 0; i < TOK; ++i) {
                 const int tok = tok0 + i;
                 if (tok < L) {
                     out[(base + (long)tok * sg.tok_stride) * CH + c] = acc[i];
-                    s1 += acc[i];
-                    s2 = fmaf(acc[i], acc[i], s2);
+                    if (!RAGGED) {
+                        const float d = acc[i] - piv;
+                        s1 += d;
+                        s2 = fmaf(d, d, s2);
+                    }
                 }
             }
             store_chunk<false>(regs, U, nullptr, nullptr, k + 2);
@@ -146,13 +157,18 @@ __global__ void __launch_bounds__(256, 3) glu_dwconv_fwd_kernel(const float* __r
         }
         tile += kend - k0;
     }
-    if (bn_sums) {
+    if (!RAGGED && bn_sums) {
+        // back to raw sums in double (sum y = s' + n p, sum y^2 = q' + 2 p s' + n p^2) before the halves are combined: the sums layout and
+        // cmgan_norm_finalize stay as they are
+        const double pd = piv, sd = s1;
+        const double t1 = sd + cnt * pd, t2 = (double)s2 + 2.0 * pd * sd + cnt * pd * pd;
+        double* UD = reinterpret_cast<double*>(U);
         __syncthreads();
-        if (half) { U[c] = s1; U[CH + c] = s2; }
+        if (half) { UD[c] = t1; UD[CH + c] = t2; }
         __syncthreads();
         if (!half) {
-            atomicAdd(bn_sums + c * 2, (double)s1 + (double)U[c]);
-            atomicAdd(bn_sums + c * 2 + 1, (double)s2 + (double)U[CH + c]);
+            atomicAdd(bn_sums + c * 2, t1 + UD[c]);
+            atomicAdd(bn_sums + c * 2 + 1, t2 + UD[CH + c]);
         }
     }
 }

@@ -13,13 +13,11 @@ Conventions of the file:
   * inputs sit on the edges on purpose: PReLU inputs exactly 0, complex magnitudes exactly 0, max-pool ties and NaNs, row counts that are
     not multiples of the launch tiles, strided views wherever the ABI takes strides.
 """
-import math
-
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from f64_check import DEV, EPS, NAN, SENT, TAIL, _buf, _cdiv, _close, _exact, _f32, _gen, _mix_seed, _randn, _tail, _unif
 from tf32_model import tf32_rna
 
 pytestmark = pytest.mark.gpu
@@ -27,71 +25,6 @@ pytestmark = pytest.mark.gpu
 if torch.cuda.is_available():
     from cmgan_b200 import ops
     from cmgan_b200.ops import call
-DEV = "cuda"
-U = 2.0 ** -24          # unit roundoff of float32
-TAIL = 64
-SENT = -12345.5         # guard value (exact in float32)
-NAN = float("nan")
-EPS = 1e-5
-
-
-def _gen(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def _randn(*shape, seed, scale=1.0):
-    return torch.randn(*shape, generator=_gen(seed)) * scale
-
-
-def _unif(*shape, seed, lo, hi):
-    return lo + (hi - lo) * torch.rand(*shape, generator=_gen(seed))
-
-
-def _f32(v):
-    """the float32 value a C ``float`` argument receives"""
-    return float(np.float32(v))
-
-
-def _cdiv(a, b):
-    return -(-a // b)
-
-
-def _buf(n, fill=NAN, dtype=torch.float32):
-    """device buffer: n elements set to ``fill`` (a scalar or a tensor of n values), then TAIL guard elements set to SENT"""
-    b = torch.full((n + TAIL,), SENT, dtype=dtype, device=DEV)
-    b[:n] = fill.reshape(-1).to(device=DEV, dtype=dtype) if isinstance(fill, torch.Tensor) else fill
-    return b
-
-
-def _tail(b, n, name):
-    t = b[n:].cpu()
-    assert torch.equal(t, torch.full_like(t, SENT)), f"{name}: the guard tail changed (write past the end)"
-
-
-def _close(got, ref, ref_abs, c, name, where=None):
-    """element-wise |got - ref| <= c 2^-24 ref_abs (c a number or a tensor); NaN anywhere fails; ``where`` restricts the check"""
-    ref = ref.detach().double().cpu()
-    got = got.detach().double().cpu().reshape(ref.shape)
-    ref_abs = ref_abs.detach().double().cpu().expand(ref.shape)
-    lim = (c * U * ref_abs) if not isinstance(c, torch.Tensor) else c.double().cpu() * U * ref_abs
-    lim = lim.expand(ref.shape)
-    if where is not None:
-        got, ref, lim = got[where], ref[where], lim[where]
-    assert torch.isfinite(ref).all(), f"{name}: the reference is not finite"
-    err = (got - ref).abs()
-    ok = err <= lim
-    if ok.numel():
-        ratio = torch.where(torch.isnan(err), torch.full_like(err, math.inf), err / lim.clamp_min(1e-300))
-        k = int(ratio.argmax())
-        print(f"[f64] {name}: {ok.numel()} elements, worst err / bound {ratio.reshape(-1)[k].item():.3g} "
-              f"(err {err.reshape(-1)[k].item():.3e})")
-        assert bool(ok.all()), (f"{name}: {int((~ok).sum())} of {ok.numel()} elements out of bound; element {k}: got "
-                                f"{got.reshape(-1)[k].item():.9g}, ref {ref.reshape(-1)[k].item():.9g}, bound {lim.reshape(-1)[k].item():.3e}")
-
-
-def _exact(got, ref, name):
-    got = got.detach().cpu().reshape(ref.shape)
-    assert torch.equal(got.view(torch.int32), ref.detach().float().contiguous().view(torch.int32)), f"{name}: not bit-identical"
 
 
 def _kink_affine(B, C, seed):
@@ -102,15 +35,6 @@ def _kink_affine(B, C, seed):
     scale = torch.randint(8, 41, (B, C), generator=g).float() / 16
     m0 = torch.round(torch.randn(B, C, generator=g) * 1024).clamp(-8191, 8191) / 1024
     return scale, -(m0 * scale), m0
-
-
-def _mix_seed(seed, counter):
-    """the effective dropout seed when a device counter is given (cmgan_mix_seed, a splitmix64 finaliser of seed and counter)"""
-    m = (1 << 64) - 1
-    z = (seed ^ (counter * 0x9E3779B97F4A7C15)) & m
-    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & m
-    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & m
-    return z ^ (z >> 31)
 
 
 # ================================================================================================ generator output heads
