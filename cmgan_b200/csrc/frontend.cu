@@ -872,3 +872,35 @@ CMGAN_API int cmgan_ola_div_bwd(const float* dy, long long lddy, int B, int T, c
     ola_div_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dy, lddy, T, inv_env, c_div, y, ldy, dframes, dc);
     return cmgan_check_launch("ola_div_bwd_kernel");
 }
+
+// ------------------------------------------------------------------ training batch cut (dataloader.py:32-49) on the device
+namespace {
+
+__global__ void cut_batch_kernel(const float* __restrict__ corpus, const long long* __restrict__ offsets, const int* __restrict__ lengths,
+                                 const int* __restrict__ starts, int cut_len, float* __restrict__ out, long long ldo) {
+    const int b = blockIdx.y;
+    const long long off = offsets[b];
+    const int len = lengths[b];
+    const int start = len >= cut_len ? min(max(starts[b], 0), len - cut_len) : 0;
+    float* o = out + (long long)b * ldo;
+    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < cut_len; n += gridDim.x * blockDim.x) {
+        float v = 0.f;
+        if (len > 0) v = len < cut_len ? corpus[off + n % len] : corpus[off + start + n];
+        o[n] = v;
+    }
+}
+
+}  // namespace
+
+// out[b, :cut_len] from utterance b = corpus[offsets[b] : offsets[b] + lengths[b]]: shorter utterances repeat whole and end with their first
+// cut_len % len samples, longer ones give cut_len samples from starts[b] clamped to [0, len - cut_len]; len <= 0 gives zeros
+CMGAN_API int cmgan_cut_batch(const float* corpus, const long long* offsets, const int* lengths, const int* starts, int B, int cut_len, float* out,
+                              long long ldo, void* stream) {
+    CMGAN_REQUIRE(corpus && offsets && lengths && starts && out, "cmgan_cut_batch: null pointer");
+    CMGAN_REQUIRE(B > 0 && cut_len > 0, "cmgan_cut_batch: B and cut_len must be positive (B=%d cut_len=%d)", B, cut_len);
+    CMGAN_REQUIRE(ldo >= cut_len, "cmgan_cut_batch: ldo=%lld is shorter than cut_len=%d", ldo, cut_len);
+    CMGAN_REQUIRE(B <= 65535, "cmgan_cut_batch: B=%d exceeds 65535 rows", B);
+    dim3 grid(min(cdiv(cut_len, 256), 1024), B);
+    cut_batch_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(corpus, offsets, lengths, starts, cut_len, out, ldo);
+    return cmgan_check_launch("cut_batch_kernel");
+}

@@ -768,6 +768,24 @@ static int train_setup(Run& r, Saved& sv, const char* who, const float* params, 
     return 0;
 }
 
+// the backward call's first half: a forward walk that launches nothing and only places the saved activations where the forward call left them
+static int place_saved(Run& r, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F) {
+    r.quiet = true;
+    forward(r, x, sxb, sxc, sxt, sxf, B, T, F, nullptr, nullptr);
+    r.quiet = false;
+    r.top = r.peak = 0;
+    return r.rc;
+}
+
+// the backward walk from the scratch position `r` is at; grads null = frozen weights
+static void backward_pass(Run& r, const Saved& sv, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
+                          const float* dfr, const float* dfi, long long sgb, long long sgt, long long sgf, float* grads, float* dx) {
+    float* gscratch = r.alloc((size_t)table().total);       // frozen weights: the gradient atomics fused into the data-gradient kernels land here
+    r.G = grads ? grads : gscratch;
+    r.wgrad = grads != nullptr;
+    backward(r, sv, x, sxb, sxc, sxt, sxf, B, T, F, dfr, dfi, sgb, sgt, sgf, dx);
+}
+
 CMGAN_API int cmgan_tscnet_fwd_train(float* params, const float* x, long long sxb, long long sxc, long long sxt, long long sxf, int B, int T, int F,
                                      int training, unsigned long long seed, const unsigned long long* seed_dev, float* final_real, float* final_imag,
                                      void* workspace, long long workspace_bytes, int precision, void* stream) {
@@ -793,15 +811,206 @@ CMGAN_API int cmgan_tscnet_bwd(const float* params, const float* x, long long sx
     Run r;
     Saved sv;
     if (train_setup(r, sv, who, params, x, B, T, F, training, seed, seed_dev, workspace, workspace_bytes, precision, stream) != 0) return -1;
-    r.quiet = true;          // the forward walk launches nothing here: it only places the saved activations where the forward call left them
-    forward(r, x, sxb, sxc, sxt, sxf, B, T, F, nullptr, nullptr);
-    if (r.rc != 0) return r.rc;
-    r.quiet = false;
-    r.top = r.peak = 0;
-    float* gscratch = r.alloc((size_t)table().total);       // frozen weights: the gradient atomics fused into the data-gradient kernels land here
-    r.G = grads ? grads : gscratch;
-    r.wgrad = grads != nullptr;
-    r.P = params;
-    backward(r, sv, x, sxb, sxc, sxt, sxf, B, T, F, dfr, dfi, sgb, sgt, sgf, dx);
+    if (place_saved(r, x, sxb, sxc, sxt, sxf, B, T, F) != 0) return r.rc;
+    backward_pass(r, sv, x, sxb, sxc, sxt, sxf, B, T, F, dfr, dfi, sgb, sgt, sgf, grads, dx);
+    return r.rc;
+}
+
+// ==================================================================================== training from waveforms (train.py:72-151)
+// The launch sequence of FusedTrainer.generator_step around the TSCNet pair: RMS scale, the STFT front end of both batches, the TSCNet
+// forward, the inverse STFT, the spectral and time-domain losses; then the magnitude term's gradient, the inverse STFT's backward and the
+// TSCNet backward.  Workspace: the waveform region first, then TSCNet's training layout (saved region, scratch).  The front end and the
+// inverse STFT (and its backward) take their scratch from TSCNet's scratch area: nothing of TSCNet's is live there at those points.
+namespace {
+
+// what the waveform ends keep across the TSCNet forward or for the backward: the STFT tables, the RMS scales, both compressed spectrograms
+// (the noisy one is TSCNet's x), fr / fi, the spectral-loss gradients and the time-loss gradient d_audio (B, Lo)
+struct WaveKeep { float *fwd, *inv, *env, *c, *xn, *xc, *fr, *fi, *der, *dei, *dau; };
+
+// places the region at k's base (k.dry: sizes it only); returns its size rounded up to 256 bytes
+size_t wave_keep(Run& k, int B, int T, WaveKeep& w) {
+    const size_t MT = (size_t)B * T, F = NFEAT;
+    w.fwd = k.alloc((size_t)NFFT * 2 * F);
+    w.inv = k.alloc((size_t)2 * F * NFFT);
+    w.env = k.alloc((size_t)HOP * (T - 1));
+    w.c = k.alloc(B);
+    w.xn = k.alloc(MT * 2 * F);
+    w.xc = k.alloc(MT * 2 * F);
+    w.fr = k.alloc(MT * F);
+    w.fi = k.alloc(MT * F);
+    w.der = k.alloc(MT * F);
+    w.dei = k.alloc(MT * F);
+    w.dau = k.alloc((size_t)B * HOP * (T - 1));
+    return (k.top + 255) & ~(size_t)255;
+}
+
+struct WaveArgs {
+    const float *clean, *noisy;
+    long long ldc, ldn;
+    float w_ri, w_mag, w_t;
+    float *est_audio, *est_mag, *clean_mag;
+    long long lde;
+    double* acc;
+};
+
+void gen_wave_fwd_walk(Run& r, const WaveKeep& w, int B, int L, const WaveArgs& a) {
+    const int T = L / HOP + 1, F = NFEAT, Lo = HOP * (T - 1), Lp = (L + NFFT + HOP - 1) / HOP * HOP;
+    const long long MT = (long long)B * T, TF = (long long)T * F;
+    if (r.live()) r.ok(cmgan_stft_tables(w.fwd, w.inv, T, w.env, nullptr, r.st));
+    if (r.live()) r.ok(cmgan_rms_scale(a.noisy, a.ldn, B, L, w.c, r.st));
+    // signal.stft_compress of the noisy batch, then of the clean batch, both scaled by the noisy batch's c (train.py:75-79); exact fp32 DFTs
+    const float* src[2] = {a.noisy, a.clean};
+    const long long lds[2] = {a.ldn, a.ldc};
+    float* dst[2] = {w.xn, w.xc};
+    const size_t mark = r.top;
+    for (int i = 0; i < 2; ++i) {
+        float* xp = r.alloc((size_t)B * Lp);
+        float* S = r.alloc((size_t)MT * 2 * F);
+        if (r.live()) r.ok(cmgan_pad_reflect(src[i], lds[i], B, L, w.c, xp, Lp, r.st));
+        Gemm(xp, HOP, w.fwd, 0, 2 * F, 1, nullptr, S, 2 * F, MT, 2 * F, NFFT).conv(1, T, 1, Lp / HOP).precision(0).run(r);
+        if (r.live()) r.ok(cmgan_compress(S, B, T, dst[i], r.st));
+        r.top = mark;
+    }
+    forward(r, w.xn, 2 * TF, TF, F, 1, B, T, F, w.fr, w.fi);
+    r.top = mark;
+    // signal.uncompress_istft_fwd without de-normalisation: est_audio stays at the RMS-scaled level (train.py:106-112)
+    float* U = r.alloc((size_t)MT * 2 * F);
+    float* frames = r.alloc((size_t)MT * NFFT);
+    float* ea = r.alloc((size_t)B * Lo);
+    if (r.live()) r.ok(cmgan_uncompress(w.fr, w.fi, TF, F, 1, B, T, U, r.st));
+    Gemm(U, 2 * F, w.inv, 0, NFFT, 1, nullptr, frames, NFFT, MT, NFFT, 2 * F).precision(0).run(r);
+    if (r.live()) r.ok(cmgan_ola(frames, B, T, w.env, nullptr, ea, Lo, r.st));
+    r.zero(a.acc, 3 * sizeof(double));
+    if (r.live())
+        r.ok(cmgan_spec_loss(w.fr, w.fi, w.xc, w.xc + TF, TF, 2 * TF, MT * F, a.w_ri, a.w_mag, a.acc, w.der, w.dei, a.est_mag, a.clean_mag, r.st));
+    // against the un-scaled clean batch, as the reference's train_step stores it (train.py:188)
+    if (r.live()) r.ok(cmgan_time_loss(ea, Lo, a.clean, a.ldc, B, Lo, a.w_t, a.acc, w.dau, r.st));
+    if (r.live()) {          // d_audio keeps the row stride Lo whatever lde is: est_audio leaves the workspace by one 2-D copy
+        const cudaError_t e = cudaMemcpy2DAsync(a.est_audio, (size_t)a.lde * 4, ea, (size_t)Lo * 4, (size_t)Lo * 4, B, cudaMemcpyDeviceToDevice, r.st);
+        if (e != cudaSuccess) { cmgan_set_error("%s: cudaMemcpy2DAsync: %s", r.who, cudaGetErrorString(e)); r.rc = -1; }
+    }
+    r.top = mark;
+}
+
+// d_mag (B, 1, F, T) with element strides (sgb, sgt, sgf), or null
+void gen_wave_bwd_walk(Run& r, const Saved& sv, const WaveKeep& w, int B, int T, const float* d_mag, long long sgb, long long sgt, long long sgf,
+                       float* grads) {
+    const int F = NFEAT, Lo = HOP * (T - 1);
+    const long long MT = (long long)B * T, TF = (long long)T * F;
+    if (d_mag && r.live()) r.ok(cmgan_mag_bwd_add(w.fr, w.fi, d_mag, sgb, sgt, sgf, B, T, F, w.der, w.dei, r.st));
+    // signal.uncompress_istft_bwd, accumulated into the spectral-loss gradients
+    const size_t mark = r.top;
+    float* dframes = r.alloc((size_t)MT * NFFT);
+    float* dU = r.alloc((size_t)MT * 2 * F);
+    if (r.live()) r.ok(cmgan_ola_bwd(w.dau, Lo, B, T, w.env, dframes, r.st));
+    Gemm(dframes, NFFT, w.inv, 0, 1, NFFT, nullptr, dU, 2 * F, MT, 2 * F, NFFT).precision(0).run(r);
+    if (r.live()) r.ok(cmgan_uncompress_bwd(w.fr, w.fi, TF, F, 1, B, T, dU, w.der, w.dei, 1, r.st));
+    r.top = mark;
+    backward_pass(r, sv, w.xn, 2 * TF, TF, F, 1, B, T, F, w.der, w.dei, TF, F, 1, grads, nullptr);
+}
+
+struct WaveLayout { size_t wave; TrainLayout t; };
+
+// an exact dry run of both walks
+WaveLayout wave_layout(int B, int L, int precision, bool training) {
+    const int T = L / HOP + 1;
+    WaveKeep w;
+    Run k;
+    const size_t wave = wave_keep(k, B, T, w);
+    Saved sv;
+    Run f;
+    f.P = nullptr; f.ws = nullptr; f.dry = true; f.precision = precision; f.st = nullptr; f.sv = &sv; f.saving = true; f.training = training;
+    WaveArgs a{};
+    a.lde = a.ldc = a.ldn = L;
+    gen_wave_fwd_walk(f, w, B, L, a);
+    Run b;
+    b.P = nullptr; b.ws = nullptr; b.dry = true; b.precision = precision; b.st = nullptr; b.training = training;
+    gen_wave_bwd_walk(b, sv, w, B, T, nullptr, 0, 0, 0, nullptr);
+    return {wave, {(f.ktop + 255) & ~(size_t)255, f.peak, b.peak}};
+}
+
+int wave_shape_check(const char* who, int B, int L, int precision) {
+    CMGAN_REQUIRE(B > 0, "%s: B must be positive (B=%d)", who, B);
+    CMGAN_REQUIRE(L > NFFT / 2, "%s: L=%d samples; a clip needs more than the 200-sample reflect padding of the STFT", who, L);
+    CMGAN_REQUIRE(precision == 0 || precision == 1, "%s: precision must be 0 (fp32) or 1 (tf32)", who);
+    const long long T = L / HOP + 1, elems = (long long)B * T * NFEAT * CAT;
+    CMGAN_REQUIRE(elems < (1ll << 31), "%s: B * T * 201 * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split the "
+                  "batch", who, CAT, elems);
+    return 0;
+}
+
+long long wave_bytes(int B, int L, int precision) {
+    const WaveLayout l = wave_layout(B, L, precision, true);      // eval mode keeps the same buffers and needs less statistics scratch
+    return (long long)(l.wave + l.t.keep + std::max(l.t.fwd, l.t.bwd)) + 256;
+}
+
+// checks shared by both entries; on success `r` walks the workspace (waveform region `w`, TSCNet's saved region, scratch)
+int wave_setup(Run& r, Saved& sv, WaveKeep& w, const char* who, const float* params, int B, int L, int training, unsigned long long seed,
+               const unsigned long long* seed_dev, void* workspace, long long workspace_bytes, int precision, void* stream) {
+    CMGAN_REQUIRE(params && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    if (wave_shape_check(who, B, L, precision) != 0) return -1;
+    CMGAN_REQUIRE(training == 0 || training == 1, "%s: training must be 0 (eval) or 1 (train)", who);
+    const long long need = wave_bytes(B, L, precision);
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    const WaveLayout l = wave_layout(B, L, precision, training == 1);
+    cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
+    Run k;
+    k.dry = false; k.ws = static_cast<char*>(workspace); k.cap = (size_t)workspace_bytes;
+    wave_keep(k, B, L / HOP + 1, w);
+    r.P = params; r.dry = false; r.precision = precision; r.st = (cudaStream_t)stream; r.who = who;
+    r.sv = &sv; r.saving = true; r.kws = static_cast<char*>(workspace) + l.wave;
+    r.ws = r.kws + l.t.keep; r.cap = (size_t)workspace_bytes - l.wave - l.t.keep;
+    r.training = training == 1; r.seed = seed; r.seed_dev = seed_dev;
+    return 0;
+}
+
+}  // namespace
+
+CMGAN_API long long cmgan_gen_wave_workspace_bytes(int B, int L, int precision) {
+    if (wave_shape_check("cmgan_gen_wave_workspace_bytes", B, L, precision) != 0) return -1;
+    return wave_bytes(B, L, precision);
+}
+
+CMGAN_API int cmgan_gen_wave_fwd(float* params, const float* clean, long long ldc, const float* noisy, long long ldn, int B, int L, int training,
+                                 unsigned long long seed, const unsigned long long* seed_dev, float w_ri, float w_mag, float w_t, float* est_audio,
+                                 long long lde, float* est_mag, float* clean_mag, double* acc, void* workspace, long long workspace_bytes,
+                                 int precision, void* stream) {
+    const char* who = "cmgan_gen_wave_fwd";
+    CMGAN_REQUIRE(clean && noisy && est_audio && est_mag && clean_mag && acc, "%s: null pointer", who);
+    const int Lo = L / HOP * HOP;
+    CMGAN_REQUIRE(ldc >= L && ldn >= L && lde >= Lo, "%s: row strides must cover a row (L=%d Lo=%d ldc=%lld ldn=%lld lde=%lld)", who, L, Lo, ldc, ldn,
+                  lde);
+    if (B > 0 && L > 0) {
+        const uintptr_t e0 = (uintptr_t)est_audio, e1 = (uintptr_t)(est_audio + (B - 1) * lde + Lo);
+        for (const auto& s : {std::make_pair(clean, ldc), std::make_pair(noisy, ldn)}) {
+            const uintptr_t s0 = (uintptr_t)s.first, s1 = (uintptr_t)(s.first + (B - 1) * s.second + L);
+            CMGAN_REQUIRE(e1 <= s0 || s1 <= e0, "%s: est_audio overlaps clean or noisy", who);
+        }
+    }
+    Run r;
+    Saved sv;
+    WaveKeep w;
+    if (wave_setup(r, sv, w, who, params, B, L, training, seed, seed_dev, workspace, workspace_bytes, precision, stream) != 0) return -1;
+    WaveArgs a{clean, noisy, ldc, ldn, w_ri, w_mag, w_t, est_audio, est_mag, clean_mag, lde, acc};
+    gen_wave_fwd_walk(r, w, B, L, a);
+    return r.rc;
+}
+
+CMGAN_API int cmgan_gen_wave_bwd(const float* params, int B, int L, int training, unsigned long long seed, const unsigned long long* seed_dev,
+                                 const float* d_mag, long long sgb, long long sgt, long long sgf, float* grads, void* workspace, long long workspace_bytes,
+                                 int precision, void* stream) {
+    const char* who = "cmgan_gen_wave_bwd";
+    CMGAN_REQUIRE(grads, "%s: null pointer (grads)", who);
+    CMGAN_REQUIRE((((uintptr_t)grads) & 15) == 0, "%s: grads must be 16-byte aligned", who);
+    CMGAN_REQUIRE(sgb >= 0 && sgt >= 0 && sgf >= 0, "%s: d_mag strides must be non-negative", who);
+    Run r;
+    Saved sv;
+    WaveKeep w;
+    if (wave_setup(r, sv, w, who, params, B, L, training, seed, seed_dev, workspace, workspace_bytes, precision, stream) != 0) return -1;
+    const int T = L / HOP + 1;
+    const long long TF = (long long)T * NFEAT;
+    if (place_saved(r, w.xn, 2 * TF, TF, NFEAT, 1, B, T, NFEAT) != 0) return r.rc;
+    gen_wave_bwd_walk(r, sv, w, B, T, d_mag, sgb, sgt, sgf, grads);
     return r.rc;
 }

@@ -4,8 +4,10 @@
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
 out.  ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
 parameter and input gradients.  ``cmgan_disc_fwd`` / ``cmgan_disc_bwd`` are the same pair for the metric discriminator (ref: discriminator.py:29-64),
-with the spectral-norm power iteration, parameter gradients through the spectral norm and input gradients.  torch is used here only to own
-the device memory."""
+with the spectral-norm power iteration, parameter gradients through the spectral norm and input gradients.  ``cmgan_gen_wave_fwd`` /
+``cmgan_gen_wave_bwd`` wrap the TSCNet pair in the STFT front end, the inverse STFT and the spectral and time-domain losses (ref:
+train.py:72-151), and ``cmgan_cut_batch`` cuts training batches from a corpus on the device (ref: dataloader.py:32-49).  torch is used here
+only to own the device memory."""
 from __future__ import annotations
 
 import ctypes
@@ -206,3 +208,60 @@ def disc_backward(flat: torch.Tensor, dout: torch.Tensor, shape, grads: torch.Te
     lib().call("cmgan_disc_bwd", flat.data_ptr(), B, H, W, int(bool(training)), seed & 0xFFFFFFFFFFFFFFFF, _ptr(seed_dev), dout.data_ptr(), _ptr(grads),
                _ptr(dx), _ptr(dy), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
     return dx, dy
+
+
+# ---- training from waveforms: cmgan_gen_wave_fwd / cmgan_gen_wave_bwd around the TSCNet pair, and the data loader's cut (cmgan_cut_batch)
+def gen_wave_workspace_bytes(B: int, L: int, precision: int) -> int:
+    """workspace of one ``cmgan_gen_wave_fwd`` + ``cmgan_gen_wave_bwd`` pair (the same size for train and eval mode)"""
+    n = lib().cdll.cmgan_gen_wave_workspace_bytes(B, L, precision)
+    if n < 0:
+        raise RuntimeError(lib().cdll.cmgan_last_error().decode())
+    return n
+
+
+def gen_wave_forward(flat: torch.Tensor, clean: torch.Tensor, noisy: torch.Tensor, training: bool, seed: int, seed_dev: torch.Tensor = None,
+                     precision: int = 1, workspace: torch.Tensor = None, weights=(0.1, 0.9, 0.2)):
+    """``cmgan_gen_wave_fwd``: clean / noisy (B, L) waveforms on the GPU (unit column stride) -> (est_audio (B, Lo), est_mag, clean_mag (each
+    (B, 1, T, 201)), acc (3 float64 loss sums), workspace), Lo = 100 (L // 100), T = L // 100 + 1.  ``training`` / ``seed`` / ``seed_dev`` as
+    ``tscnet_forward_train`` (the running statistics in ``flat`` are updated in place in train mode); ``weights`` = (w_ri, w_mag, w_t).  The
+    matching ``gen_wave_backward`` takes the workspace."""
+    assert clean.is_cuda and noisy.is_cuda and flat.is_cuda and clean.dim() == 2 and clean.shape == noisy.shape
+    assert clean.dtype == torch.float32 and noisy.dtype == torch.float32 and clean.stride(1) == 1 and noisy.stride(1) == 1
+    B, L = noisy.shape
+    T, Lo = L // 100 + 1, L // 100 * 100
+    if workspace is None:
+        workspace = torch.empty(gen_wave_workspace_bytes(B, L, precision), dtype=torch.uint8, device=noisy.device)
+    est_audio = torch.empty(B, Lo, device=noisy.device)
+    est_mag, clean_mag = torch.empty(B, 1, T, 201, device=noisy.device), torch.empty(B, 1, T, 201, device=noisy.device)
+    acc = torch.empty(3, dtype=torch.float64, device=noisy.device)
+    lib().call("cmgan_gen_wave_fwd", flat.data_ptr(), clean.data_ptr(), clean.stride(0), noisy.data_ptr(), noisy.stride(0), B, L, int(bool(training)),
+               seed & 0xFFFFFFFFFFFFFFFF, _ptr(seed_dev), float(weights[0]), float(weights[1]), float(weights[2]), est_audio.data_ptr(),
+               est_audio.stride(0), est_mag.data_ptr(), clean_mag.data_ptr(), acc.data_ptr(), workspace.data_ptr(), workspace.numel(), precision,
+               torch.cuda.current_stream().cuda_stream)
+    return est_audio, est_mag, clean_mag, acc, workspace
+
+
+def gen_wave_backward(flat: torch.Tensor, shape, d_mag, grads: torch.Tensor, *, training: bool, seed: int, seed_dev: torch.Tensor = None,
+                      precision: int = 1, workspace: torch.Tensor):
+    """``cmgan_gen_wave_bwd`` after ``gen_wave_forward`` with the same shape ((B, L) of the waveform batch), flat, training, seed, seed_dev,
+    precision and workspace.  d_mag: gradient wrt est_mag as a (B, 1, 201, T) tensor of any strides (the discriminator's input gradient), or
+    None.  The parameter gradients are accumulated into ``grads`` (laid out like ``flat``)."""
+    B, L = shape
+    assert grads is not None and grads.is_cuda
+    gs = (0, 0, 0, 0) if d_mag is None else d_mag.stride()
+    lib().call("cmgan_gen_wave_bwd", flat.data_ptr(), B, L, int(bool(training)), seed & 0xFFFFFFFFFFFFFFFF, _ptr(seed_dev), _ptr(d_mag), gs[0], gs[3],
+               gs[2], grads.data_ptr(), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+
+
+def cut_batch(corpus: torch.Tensor, offsets: torch.Tensor, lengths: torch.Tensor, starts: torch.Tensor, cut_len: int, out: torch.Tensor = None):
+    """``cmgan_cut_batch``: rows of ``cut_len`` samples cut from the packed corpus (1-D fp32 on the GPU) as the data loader cuts them;
+    offsets (int64), lengths and starts (int32) are (B,) device tensors.  Returns ``out`` (B, cut_len)."""
+    B = offsets.numel()
+    assert offsets.dtype == torch.int64 and lengths.dtype == torch.int32 and starts.dtype == torch.int32
+    assert lengths.numel() == B and starts.numel() == B and corpus.dtype == torch.float32
+    if out is None:
+        out = torch.empty(B, cut_len, device=corpus.device)
+    assert out.stride(1) == 1 and tuple(out.shape) == (B, cut_len)
+    lib().call("cmgan_cut_batch", corpus.data_ptr(), offsets.contiguous().data_ptr(), lengths.contiguous().data_ptr(), starts.contiguous().data_ptr(),
+               B, cut_len, out.data_ptr(), out.stride(0), torch.cuda.current_stream().cuda_stream)
+    return out

@@ -204,6 +204,35 @@ long long cmgan_disc_workspace_bytes(int B, int H, int W, int precision);
 int cmgan_disc_fwd(float* params, const float* x, long long sxb, long long sxh, long long sxw, const float* y, long long syb, long long syh, long long syw, int B, int H, int W, int training, unsigned long long seed, const unsigned long long* seed_dev, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
 int cmgan_disc_bwd(const float* params, int B, int H, int W, int training, unsigned long long seed, const unsigned long long* seed_dev, const float* dout, float* grads, float* dx, float* dy, void* workspace, long long workspace_bytes, int precision, void* stream);
 
+/* ---- module level, training from waveforms: the generator's side of train.py:72-151 around the TSCNet pair above, one call each way.
+ * cmgan_gen_wave_fwd: clean, noisy (B, L) fp32 with row strides ldc, ldn >= L.  Runs: c = the noisy batch's RMS scale; the STFT (n_fft 400,
+ *   hop 100, exact fp32) and power compression of the noisy and of the clean batch, both scaled by c; TSCNet.forward on the noisy spectrogram
+ *   (training / seed / seed_dev / params as cmgan_tscnet_fwd_train, running statistics updated in place in train mode); un-compression and the
+ *   inverse STFT into est_audio (B, Lo), Lo = 100 floor(L / 100), row stride lde >= Lo, left at the RMS-scaled level; the spectral loss
+ *   (cmgan_spec_loss with w_ri, w_mag), writing est_mag and clean_mag as contiguous (B, 1, T, 201), T = L / 100 + 1; the time loss (cmgan_time_loss
+ *   with w_t) of est_audio against the UN-scaled clean[:, :Lo], as the reference's train_step compares them (train.py:188).  acc (3 doubles) is
+ *   zeroed by the call and holds the loss sums cmgan_gen_loss_finalize(acc, B * T * 201, B * Lo, ...) turns into the loss.
+ * Between the two calls the host runs the GAN term: cmgan_disc_fwd on (B, 1, 201, T) views of clean_mag / est_mag, cmgan_gen_loss_finalize, and
+ *   cmgan_disc_bwd with grads = NULL for d_mag; without a discriminator, finalize with fake = NULL and pass d_mag = NULL.
+ * cmgan_gen_wave_bwd: d_mag, the gradient wrt est_mag in a (B, 1, 201, T) layout with element strides (sgb along B, sgt along T, sgf along F), or
+ *   NULL.  Adds the magnitude term to the spectral-loss gradients, runs the inverse STFT's backward into them and the TSCNet backward; every
+ *   parameter gradient is ACCUMULATED into grads (non-null, laid out like params; running-statistic slots never written).  No waveform gradient.
+ *   It reads only params, d_mag and the workspace: clean, noisy, est_audio, est_mag and clean_mag may have changed since the forward.  Otherwise
+ *   the preconditions of cmgan_tscnet_bwd hold: the same workspace, B, L, training, seed, precision, *seed_dev and unchanged params.
+ * The workspace (256-byte aligned, >= cmgan_gen_wave_workspace_bytes(B, L, precision), the same for both modes) starts with a region holding
+ *   the STFT tables (regenerated by every forward), the RMS scales, both compressed spectrograms, fr / fi, the spectral-loss gradients and the
+ *   time-loss gradient; TSCNet's training layout lies above it.  All three return -1 (no launch) for B <= 0, L <= 200, precision not 0 / 1, or
+ *   B * T * 201 * 320 >= 2^31; the calls also for null or misaligned pointers (params, grads 16-byte; workspace 256-byte; d_mag may be NULL),
+ *   ldc or ldn < L, lde < Lo, est_audio overlapping clean or noisy, training not 0 / 1 or a workspace smaller than the query.
+ * cmgan_cut_batch: the data loader's cut (dataloader.py:32-49) on the device.  Utterance b is corpus[offsets[b] : offsets[b] + lengths[b]]
+ *   (offsets, lengths, starts: device arrays); out[b, n], n < cut_len, row stride ldo >= cut_len, is corpus[off + n % len] when len < cut_len
+ *   (whole copies, then the first cut_len % len samples), else corpus[off + start + n] with start = starts[b] clamped to [0, len - cut_len]; a
+ *   row with len <= 0 is zero-filled.  Nothing outside an utterance is read.  Call it once for the clean and once for the noisy corpus. */
+long long cmgan_gen_wave_workspace_bytes(int B, int L, int precision);
+int cmgan_gen_wave_fwd(float* params, const float* clean, long long ldc, const float* noisy, long long ldn, int B, int L, int training, unsigned long long seed, const unsigned long long* seed_dev, float w_ri, float w_mag, float w_t, float* est_audio, long long lde, float* est_mag, float* clean_mag, double* acc, void* workspace, long long workspace_bytes, int precision, void* stream);
+int cmgan_gen_wave_bwd(const float* params, int B, int L, int training, unsigned long long seed, const unsigned long long* seed_dev, const float* d_mag, long long sgb, long long sgt, long long sgf, float* grads, void* workspace, long long workspace_bytes, int precision, void* stream);
+int cmgan_cut_batch(const float* corpus, const long long* offsets, const int* lengths, const int* starts, int B, int cut_len, float* out, long long ldo, void* stream);
+
 /* ---- module level, waveform in / waveform out: evaluation.py:21-53 (enhance_one_track between load and save) as one call.
  * wav (B, L) fp32 with row stride ldw; out (B, L) fp32 with row stride ldo; neither range may overlap the other.  Per clip: RMS scale,
  * wrap padding to a multiple of 100, the STFT, power compression, TSCNet.forward (params / precision as cmgan_tscnet_fwd), un-compression,
