@@ -252,8 +252,12 @@ __global__ void __launch_bounds__(128) attn_fwd_mma_kernel(const float* __restri
 
 
 // ============================================================================================ backward
-// Both backward kernels recompute the logits tile by tile exactly as the forward does (tf32 operands, fp32 accumulate) and use
+// Both backward kernels recompute the logits tile by tile (tf32 operands, fp32 accumulate) and use
 //   p = exp2(s - lse),  dp = dO V^T,  ds = p (dp - delta),  delta_i = dO_i . O_i
+// The dq kernel rounds its operands as the forward does (q 0.25 log2 e rounded to nearest; K and the E window truncated by the tensor
+// core).  The dk / dv kernel holds K 0.25 log2 e and V in registers, rounded to nearest, and streams Q, dO and the E window raw, so the
+// tensor core truncates them; R2 takes Q 0.25 log2 e unrounded.  Its logits therefore differ from the forward's at the tf32 level, and
+// p = exp2(s - lse) against the forward's lse is not exactly normalised.
 // (ds is the gradient wrt the natural-log logits; q is held pre-scaled by 0.25 log2(e), so sums against q take a final ln 2).
 constexpr float LN2 = 0.6931471805599453f;
 

@@ -1,5 +1,6 @@
-"""Shared helpers of the float64 kernel checks (test_gpu_kernels_f64.py, test_gpu_dense_f64.py): guarded device buffers, the element-wise
-bound |got - ref| <= c 2^-24 ref_abs, bit-exact comparison, seeded inputs and the dropout mask function."""
+"""Shared helpers of the float64 kernel checks (test_gpu_kernels_f64.py, test_gpu_dense_f64.py, test_gpu_tf32_f64.py): guarded device
+buffers, the element-wise bound |got - ref| <= c 2^-24 ref_abs (plus the tf32 form of it), bit-exact comparison, seeded inputs and the
+dropout mask function."""
 import math
 
 import numpy as np
@@ -65,6 +66,19 @@ def _close(got, ref, ref_abs, c, name, where=None):
               f"(err {err.reshape(-1)[k].item():.3e})")
         assert bool(ok.all()), (f"{name}: {int((~ok).sum())} of {ok.numel()} elements out of bound; element {k}: got "
                                 f"{got.reshape(-1)[k].item():.9g}, ref {ref.reshape(-1)[k].item():.9g}, bound {lim.reshape(-1)[k].item():.3e}")
+
+
+def _tf32_ok(got, name):
+    """every element a tf32 value: low 13 mantissa bits zero"""
+    bits = got.detach().contiguous().cpu().view(torch.int32)
+    assert bool(((bits & 0x1FFF) == 0).all()), f"{name}: not rounded to tf32"
+
+
+def _close_tf32(got, ref, lim_u, name, where=None):
+    """the float32 bound (lim_u, in units of 2^-24) plus half a tf32 spacing of the result (rna: 2^-11 relative)"""
+    _tf32_ok(got if where is None else got.detach().cpu().reshape(ref.shape)[where], name)
+    g = got.detach().double().cpu().reshape(ref.shape)
+    _close(got, ref, lim_u.cpu().expand(ref.shape) + 2.0 ** 13 * g.abs(), 1, name, where)
 
 
 def _exact(got, ref, name):

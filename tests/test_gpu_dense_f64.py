@@ -14,7 +14,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64_check import DEV, EPS, NAN, SENT, U, _buf, _cdiv, _close, _exact, _f32, _keep, _mix_seed, _randn, _tail, _unif
+from f64_check import DEV, EPS, NAN, SENT, U, _buf, _cdiv, _close, _close_tf32, _exact, _f32, _keep, _mix_seed, _randn, _tail, _unif
 
 pytestmark = pytest.mark.gpu
 
@@ -30,19 +30,6 @@ def _nsm():
 
 def _set_rounding(on):
     lib().cdll.cmgan_set_tf32_rounding(1 if on else 0)
-
-
-def _tf32_ok(got, name):
-    """every element a tf32 value: low 13 mantissa bits zero"""
-    bits = got.detach().contiguous().cpu().view(torch.int32)
-    assert bool(((bits & 0x1FFF) == 0).all()), f"{name}: not rounded to tf32"
-
-
-def _close_tf32(got, ref, lim_u, name):
-    """the float32 bound (lim_u, in units of 2^-24) plus half a tf32 spacing of the result (rna: 2^-11 relative)"""
-    _tf32_ok(got, name)
-    g = got.detach().double().cpu().reshape(ref.shape)
-    _close(got, ref, lim_u.cpu().expand(ref.shape) + 2.0 ** 13 * g.abs(), 1, name)
 
 
 def _sig_err(b):
