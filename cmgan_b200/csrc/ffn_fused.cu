@@ -8,19 +8,15 @@
 // contraction (64 KB of shared memory; it never reaches HBM) -> wgmma into 64 x 64 -> bias, dropout, alpha, residual -> store.
 // Only the module input is kept for the backward pass.
 //
-// Backward: one kernel recomputes the hidden pre-activation h (LN + first contraction) and forms dh = (dz W2) * swish'(h) * drop1 one
+// Backward: ONE kernel.  It recomputes the hidden pre-activation h (LN + first contraction) and forms dh = (dz W2) * swish'(h) * drop1 one
 // 64-column quarter of the hidden layer at a time (two 64 x 64 accumulators in registers), writing the operands of the two weight-gradient
-// GEMMs (xn, a = swish(h) * drop1, dh) and the LayerNorm statistics; the data gradient dLN = dh W1 and the LayerNorm backward then run
-// as the library's row GEMM and LayerNorm-backward kernels.
+// GEMMs (xn, a = swish(h) * drop1, dh) and the LayerNorm statistics.  The rounded dh quarter stays in registers as the A operand of
+// dLN += dh_q W1_q (a third 64 x 64 accumulator; W1^T is the third resident 64 KB image), and the LayerNorm backward runs on that
+// accumulator in the same CTA, so neither dh nor dLN is read back from HBM.
 // Dropout masks are the counter-based hash of the GEMM epilogues (csrc/gemm_tc.cu): pair (m * N + n) / 2, 16 bits per element.
-#include <cstring>
-
 #include "common.cuh"
 #include "../../include/cmgan_b200.h"
-#include "gemm_args.h"
 #include "tc_ptx.cuh"
-
-int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st);    // gemm_tc.cu
 
 namespace {
 using namespace cmgan_tc;
@@ -82,6 +78,24 @@ __device__ __forceinline__ float2 ln_tile(const float* __restrict__ x, long ldx,
     return make_float2(mean, rstd);
 }
 
+// one 32-float K chunk (4 K steps) into 64 x (64 NB) accumulators, one m64n64k8 instruction per 64 columns: the A rows are read from
+// shared memory once per 64 columns instead of once per 16.  Same fragment layout as mma_chunk<4 NB> (acc[4 b + c] = columns 64 b + 16 c ..).
+template <int NB>
+__device__ __forceinline__ void mma_chunk64(float (&acc)[4 * NB][8], uint64_t adesc, uint64_t bdesc, bool first) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int b = 0; b < NB; ++b)
+            wgmma_m64n64k8_tf32(*reinterpret_cast<float(*)[4][8]>(&acc[4 * b]), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(512 * b + 2 * k),
+                                (first && k == 0) ? 0u : 1u);
+}
+
+// start pulling the rows [m0, m0 + 64) of an array into L2 ahead of their use: one 128-byte line per thread
+__device__ __forceinline__ void prefetch_rows_l2(const float* p, long ld, long m0, long M) {
+    const long m = m0 + (threadIdx.x >> 1);
+    if (m < M) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + m * ld + (threadIdx.x & 1) * 32));
+}
+
 struct FfnFwdArgs {
     const float* x; long long ldx; float* out; long long ldo;
     const float* ln_g; const float* ln_b; const float* W1p; const float* b1; const float* W2p; const float* b2;
@@ -105,13 +119,14 @@ __global__ void __launch_bounds__(NT, 1) ffn_fwd_kernel(const __grid_constant__ 
     const long ntiles = (g.M + BM - 1) / BM;
     for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long m0 = tile * BM;
+        prefetch_rows_l2(g.x, g.ldx, m0 + (long)gridDim.x * BM, g.M);       // the CTA's next tile
         ln_tile(g.x, g.ldx, m0, g.M, g.ln_g, g.ln_b, sXn, nullptr);
         fence_proxy_async();
         __syncthreads();
         float acc[16][8];
         wgmma_fence();
-        mma_chunk<16, 16>(acc, gmma_desc_sw128(base + 2 * W_BYTES), gmma_desc_sw128(base), true);
-        mma_chunk<16, 16>(acc, gmma_desc_sw128(base + 2 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128), false);
+        mma_chunk64<4>(acc, gmma_desc_sw128(base + 2 * W_BYTES), gmma_desc_sw128(base), true);
+        mma_chunk64<4>(acc, gmma_desc_sw128(base + 2 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128), false);
         wgmma_commit();
         wgmma_wait<0>();
         // hidden activation -> second A operand (fragment rows 16 warp + fg (+ 8), columns 16 j + 8 i + 2 ft (+ 1))
@@ -134,7 +149,7 @@ __global__ void __launch_bounds__(NT, 1) ffn_fwd_kernel(const __grid_constant__ 
         wgmma_fence();
 #pragma unroll
         for (int c = 0; c < 8; ++c)
-            mma_chunk<4, 4>(acc2, gmma_desc_sw128(base + 2 * W_BYTES + 2 * CHUNK + c * CHUNK), gmma_desc_sw128(base + W_BYTES + c * CHUNK), c == 0);
+            mma_chunk64<1>(acc2, gmma_desc_sw128(base + 2 * W_BYTES + 2 * CHUNK + c * CHUNK), gmma_desc_sw128(base + W_BYTES + c * CHUNK), c == 0);
         wgmma_commit();
         wgmma_wait<0>();
 #pragma unroll
@@ -157,34 +172,78 @@ __global__ void __launch_bounds__(NT, 1) ffn_fwd_kernel(const __grid_constant__ 
 }
 
 struct FfnBwdArgs {
-    const float* x; long long ldx; const float* dz; long long lddz;
-    const float* ln_g; const float* ln_b; const float* W1p; const float* b1; const float* W2tp;
+    const float* x; long long ldx; const float* dz; long long lddz; const float* dout; long long lddo; const float* res2; long long ldr2;
+    const float* ln_g; const float* ln_b; const float* W1p; const float* b1; const float* W2tp; const float* W1tp;
     long long M; unsigned long long seed1; unsigned int thr; float inv_keep; const unsigned long long* seed_dev;
-    float* a_out; float* dh_out; float* xn_out; float* stats;
+    float* a_out; float* dh_out; float* xn_out; float* stats; float* dx; long long lddx; float* dgamma; float* dbeta;
 };
 
+// The W1^T image (64 channel rows x 256 hidden, K-major SWIZZLE_128B) with K permuted inside each group of 8, so that the rounded dh
+// accumulator fragment is the register A operand of dLN = dh W1 as it stands: a thread holds hidden columns 2 t, 2 t + 1 of a group,
+// where the A fragment wants columns t, t + 4, so slot s of a group holds hidden column 2 s (s < 4) or 2 (s - 4) + 1.
+__device__ __forceinline__ void copy_image_kperm(uint8_t* dst, const float* __restrict__ src) {
+    for (int u = threadIdx.x; u < W_BYTES / 16; u += NT) {
+        const int c = u >> 9, n = (u >> 3) & 63, cu = u & 7;     // chunk, row, 16-byte unit (slots 4 cu .. 4 cu + 3) of the row
+        float v[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int k = 8 * (cu >> 1) + 2 * j + (cu & 1);
+            v[j] = __ldg(src + c * (CHUNK / 4) + n * 32 + (((k >> 2) ^ (n & 7)) << 2) + (k & 3));
+        }
+        *reinterpret_cast<float4*>(dst + c * CHUNK + swz(n, 4 * cu)) = make_float4(v[0], v[1], v[2], v[3]);
+    }
+}
+
+// one 64-column quarter of the hidden layer: h (acc) = xn W1^T and dz W2 (dacc) on hidden columns 64 qt .. 64 qt + 63
+__device__ __forceinline__ void bwd_quarter_mmas(float (&acc)[4][8], float (&dacc)[4][8], uint32_t base, int qt) {
+    const uint32_t wrow = (uint32_t)qt * 64 * 128;
+    mma_chunk64<1>(acc, gmma_desc_sw128(base + 3 * W_BYTES), gmma_desc_sw128(base + wrow), true);
+    mma_chunk64<1>(acc, gmma_desc_sw128(base + 3 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128 + wrow), false);
+    mma_chunk64<1>(dacc, gmma_desc_sw128(base + 3 * W_BYTES + 2 * CHUNK), gmma_desc_sw128(base + W_BYTES + wrow), true);
+    mma_chunk64<1>(dacc, gmma_desc_sw128(base + 3 * W_BYTES + 3 * CHUNK), gmma_desc_sw128(base + W_BYTES + 256 * 128 + wrow), false);
+}
+
+// Per 64-row tile: LayerNorm (xn, stats out), then per hidden quarter h and dz W2 -> a, dh out, and dLN += rna(dh) W1 with dh taken from
+// registers; the quarter's dLN MMAs are issued together with the next quarter's.  Then the LayerNorm backward on the 64 x 64 dLN
+// accumulator, row sums over the quad that holds a row: dx = rstd (dLN g - mean(dLN g) - xhat mean(dLN g xhat)) + dout (+ res2).
+// dgamma / dbeta: per-thread column partials over the CTA's tiles, reduced in the CTA, one atomic per column per CTA.
 __global__ void __launch_bounds__(NT, 1) ffn_bwd_kernel(const __grid_constant__ FfnBwdArgs g) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* const bp = smem_raw + (base - smem_u32(smem_raw));
     uint8_t* const sW1 = bp;                       // W1 image: 2 chunks x 256 rows (h = xn W1^T)
     uint8_t* const sW2t = bp + W_BYTES;            // W2^T image: 2 chunks x 256 rows (dz W2)
-    uint8_t* const sXn = bp + 2 * W_BYTES;         // 2 chunks x 64 rows
+    uint8_t* const sW1t = bp + 2 * W_BYTES;        // K-permuted W1^T image: 8 chunks x 64 rows (dLN = dh W1)
+    uint8_t* const sXn = bp + 3 * W_BYTES;         // 2 chunks x 64 rows
     uint8_t* const sDz = sXn + 2 * CHUNK;          // 2 chunks x 64 rows
+    float2* const sStats = reinterpret_cast<float2*>(sDz + 2 * CHUNK);     // 64 x (mean, rstd)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, fg = lane >> 2, ft = lane & 3;
     const bool drop_on = g.thr != 0u;
     const uint32_t thr16 = g.thr >> 16;
     const uint32_t s1 = cmgan_seed32(cmgan_eff_seed(g.seed1, g.seed_dev));
     copy_image(sW1, g.W1p, W_BYTES);
     copy_image(sW2t, g.W2tp, W_BYTES);
+    copy_image_kperm(sW1t, g.W1tp);
+    float pg[4][4], pb[4][4];                      // dgamma / dbeta partials of columns 16 j + 8 (e >> 1) + 2 ft + (e & 1)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) pg[j][e] = pb[j][e] = 0.f;
     const long ntiles = (g.M + BM - 1) / BM;
     for (long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const long m0 = tile * BM;
+        const long m0 = tile * BM, mn = m0 + (long)gridDim.x * BM;      // mn: the CTA's next tile
+        prefetch_rows_l2(g.x, g.ldx, mn, g.M);
+        prefetch_rows_l2(g.dz, g.lddz, mn, g.M);
+        prefetch_rows_l2(g.dout, g.lddo, mn, g.M);
+        if (g.res2) prefetch_rows_l2(g.res2, g.ldr2, mn, g.M);
         const float2 st = ln_tile(g.x, g.ldx, m0, g.M, g.ln_g, g.ln_b, sXn, g.xn_out);
         {   // statistics for the LayerNorm backward; dz (already a tf32 operand) -> second A operand
             const int r = threadIdx.x >> 1, half = threadIdx.x & 1;
             const long m = m0 + r;
-            if (half == 0 && m < g.M) reinterpret_cast<float2*>(g.stats)[m] = st;
+            if (half == 0) {
+                sStats[r] = st;
+                if (m < g.M) reinterpret_cast<float2*>(g.stats)[m] = st;
+            }
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
                 const float4 t = m < g.M ? __ldg(reinterpret_cast<const float4*>(g.dz + m * g.lddz + half * 32 + 4 * q)) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -193,17 +252,14 @@ __global__ void __launch_bounds__(NT, 1) ffn_bwd_kernel(const __grid_constant__ 
         }
         fence_proxy_async();
         __syncthreads();
+        float acc[4][8], dacc[4][8], dln[4][8];
+        wgmma_fence();
+        bwd_quarter_mmas(acc, dacc, base, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
 #pragma unroll 1
-        for (int qt = 0; qt < 4; ++qt) {            // hidden columns 64 qt .. 64 qt + 63
-            float acc[4][8], dacc[4][8];
-            const uint32_t wrow = (uint32_t)qt * 64 * 128;
-            wgmma_fence();
-            mma_chunk<4, 4>(acc, gmma_desc_sw128(base + 2 * W_BYTES), gmma_desc_sw128(base + wrow), true);
-            mma_chunk<4, 4>(acc, gmma_desc_sw128(base + 2 * W_BYTES + CHUNK), gmma_desc_sw128(base + 256 * 128 + wrow), false);
-            mma_chunk<4, 4>(dacc, gmma_desc_sw128(base + 2 * W_BYTES + 2 * CHUNK), gmma_desc_sw128(base + W_BYTES + wrow), true);
-            mma_chunk<4, 4>(dacc, gmma_desc_sw128(base + 2 * W_BYTES + 3 * CHUNK), gmma_desc_sw128(base + W_BYTES + 256 * 128 + wrow), false);
-            wgmma_commit();
-            wgmma_wait<0>();
+        for (int qt = 0; qt < 4; ++qt) {
+            uint32_t dha[8][4];                    // rna(dh) as the A fragments of the quarter's 8 K steps (columns permuted as sW1t)
 #pragma unroll
             for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -211,17 +267,102 @@ __global__ void __launch_bounds__(NT, 1) ffn_bwd_kernel(const __grid_constant__ 
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
                         const long m = m0 + 16 * warp + fg + 8 * hh;
-                        if (m >= g.M) continue;
                         const int n = 64 * qt + 16 * j + 8 * i + 2 * ft;
                         const float2 bb = __ldg(reinterpret_cast<const float2*>(g.b1 + n));
                         const float2 ds = drop_pair(m, n, HID, s1, thr16, g.inv_keep, drop_on);
                         const float h0 = acc[j][4 * i + 2 * hh] + bb.x, h1 = acc[j][4 * i + 2 * hh + 1] + bb.y;
+                        // rows past M have xn = dz = 0, so their dh is 0 and they add nothing to dLN
+                        const float d0 = to_tf32(dacc[j][4 * i + 2 * hh] * dswishf_(h0) * ds.x);
+                        const float d1 = to_tf32(dacc[j][4 * i + 2 * hh + 1] * dswishf_(h1) * ds.y);
+                        dha[2 * j + i][hh] = __float_as_uint(d0);
+                        dha[2 * j + i][2 + hh] = __float_as_uint(d1);
+                        if (m >= g.M) continue;
                         *reinterpret_cast<float2*>(g.a_out + m * HID + n) = make_float2(to_tf32(swishf_(h0) * ds.x), to_tf32(swishf_(h1) * ds.y));
-                        *reinterpret_cast<float2*>(g.dh_out + m * HID + n) =
-                            make_float2(to_tf32(dacc[j][4 * i + 2 * hh] * dswishf_(h0) * ds.x), to_tf32(dacc[j][4 * i + 2 * hh + 1] * dswishf_(h1) * ds.y));
+                        *reinterpret_cast<float2*>(g.dh_out + m * HID + n) = make_float2(d0, d1);
                     }
+            wgmma_fence();
+            const uint64_t bdesc = gmma_desc_sw128(base + 2 * W_BYTES + 2 * qt * CHUNK);
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk)
+                wgmma_m64n64k8_tf32_rs(dln, dha[kk], bdesc + (uint64_t)((kk >> 2) * (CHUNK >> 4) + 2 * (kk & 3)), (qt > 0 || kk > 0) ? 1u : 0u);
+            if (qt < 3) bwd_quarter_mmas(acc, dacc, base, qt + 1);
+            wgmma_commit();
+            wgmma_wait<0>();
         }
-        __syncthreads();          // sXn / sDz are rewritten by the next tile
+        // LayerNorm backward, as ln_bwd_kernel: rows 16 warp + fg + 8 hh, 16 columns per thread, the row's 64 over the quad
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const int r = 16 * warp + fg + 8 * hh;
+            const long m = m0 + r;
+            const bool ok = m < g.M;
+            const float2 s = ok ? sStats[r] : make_float2(0.f, 0.f);
+            float xh[4][4], dg[4][4], s1r = 0.f, s2r = 0.f;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int n = 16 * j + 8 * i + 2 * ft;
+                    const float2 v = ok ? __ldg(reinterpret_cast<const float2*>(g.x + m * g.ldx + n)) : make_float2(0.f, 0.f);
+                    const float2 gm = __ldg(reinterpret_cast<const float2*>(g.ln_g + n));
+                    xh[j][2 * i] = (v.x - s.x) * s.y;
+                    xh[j][2 * i + 1] = (v.y - s.x) * s.y;
+                    dg[j][2 * i] = dln[j][4 * i + 2 * hh] * gm.x;
+                    dg[j][2 * i + 1] = dln[j][4 * i + 2 * hh + 1] * gm.y;
+                    s1r += dg[j][2 * i] + dg[j][2 * i + 1];
+                    s2r += dg[j][2 * i] * xh[j][2 * i] + dg[j][2 * i + 1] * xh[j][2 * i + 1];
+                }
+            s1r += __shfl_xor_sync(0xffffffffu, s1r, 1);
+            s1r += __shfl_xor_sync(0xffffffffu, s1r, 2);
+            s2r += __shfl_xor_sync(0xffffffffu, s2r, 1);
+            s2r += __shfl_xor_sync(0xffffffffu, s2r, 2);
+            const float m1 = s1r * (1.0f / C), m2 = s2r * (1.0f / C);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int n = 16 * j + 8 * i + 2 * ft;
+                    if (ok) {
+                        float2 rr = __ldg(reinterpret_cast<const float2*>(g.dout + m * g.lddo + n));
+                        if (g.res2) {
+                            const float2 r2 = __ldg(reinterpret_cast<const float2*>(g.res2 + m * g.ldr2 + n));
+                            rr.x += r2.x; rr.y += r2.y;
+                        }
+                        *reinterpret_cast<float2*>(g.dx + m * g.lddx + n) =
+                            make_float2(s.y * (dg[j][2 * i] - m1 - xh[j][2 * i] * m2) + rr.x, s.y * (dg[j][2 * i + 1] - m1 - xh[j][2 * i + 1] * m2) + rr.y);
+                    }
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float d = dln[j][4 * i + 2 * hh + e];
+                        pg[j][2 * i + e] = fmaf(d, xh[j][2 * i + e], pg[j][2 * i + e]);
+                        pb[j][2 * i + e] += d;
+                    }
+                }
+        }
+        __syncthreads();          // sXn / sDz / sStats are rewritten by the next tile
+    }
+    // dgamma / dbeta: over the 8 row groups of the warp (butterfly), the 4 warps (in order), then one atomic per column
+    float* const red = reinterpret_cast<float*>(sXn);          // [warp][dgamma 64 | dbeta 64]
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            float a = pg[j][e], b = pb[j][e];
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+                a += __shfl_xor_sync(0xffffffffu, a, o);
+                b += __shfl_xor_sync(0xffffffffu, b, o);
+            }
+            if (fg == 0) {
+                const int n = 16 * j + 8 * (e >> 1) + 2 * ft + (e & 1);
+                red[warp * 2 * C + n] = a;
+                red[warp * 2 * C + C + n] = b;
+            }
+        }
+    __syncthreads();
+    if (threadIdx.x < C) {
+        const int n = threadIdx.x;
+        atomicAdd(g.dgamma + n, ((red[n] + red[2 * C + n]) + red[4 * C + n]) + red[6 * C + n]);
+        atomicAdd(g.dbeta + n, ((red[C + n] + red[3 * C + n]) + red[5 * C + n]) + red[7 * C + n]);
     }
 }
 
@@ -263,25 +404,18 @@ CMGAN_API int cmgan_ffn_bwd(const float* x, long long ldx, const float* dz, long
                             void* stream) {
     CMGAN_REQUIRE(x && dz && dout && ln_g && ln_b && W1p && b1 && W2tp && W1tp && dx && a_out && dh_out && xn_out && dgamma && dbeta && ws && M >= 0 &&
                   ldx % 4 == 0 && lddz % 4 == 0, "cmgan_ffn_bwd: bad arguments");
+    CMGAN_REQUIRE(lddo % 2 == 0 && (!res2 || ldr2 % 2 == 0) && lddx % 2 == 0, "cmgan_ffn_bwd: bad arguments");
     if (M == 0) return 0;
-    const size_t smem = 1024 + 2 * W_BYTES + 4 * CHUNK;
+    const size_t smem = 1024 + 3 * W_BYTES + 4 * CHUNK + BM * sizeof(float2);
     if (prepare(ffn_bwd_kernel, smem, "ffn_bwd_kernel")) return -1;
-    float* dln = ws;                 // M x 64 (16-byte aligned rows for the row GEMM)
-    float* stats = ws + C * M;       // M x (mean, rstd)
-    FfnBwdArgs a{x, ldx, dz, lddz, ln_g, ln_b, W1p, b1, W2tp, M, seed1, thr, inv_keep, seed_dev, a_out, dh_out, xn_out, stats};
-    const long ntiles = (M + BM - 1) / BM;
-    const int grid = (int)(ntiles < cmgan_num_sms() ? ntiles : cmgan_num_sms());
+    float* stats = ws + C * M;       // M x (mean, rstd); ws[0, 64 M) is unused
+    FfnBwdArgs a{x, ldx, dz, lddz, dout, lddo, res2, res2 ? ldr2 : 0, ln_g, ln_b, W1p, b1, W2tp, W1tp, M, seed1, thr, inv_keep, seed_dev,
+                 a_out, dh_out, xn_out, stats, dx, lddx, dgamma, dbeta};
+    // At most ceil(ntiles / 2) CTAs: a CTA adds the dgamma / dbeta terms of its rows in a chain of 2 T (T = its tiles) + 6 adds and one
+    // atomic, so a term sees at most 2 T + 7 + grid roundings; with grid <= ceil(M / 128) that is never longer than ln_bwd_kernel's
+    // 8 + 16 + ceil(M / 128) (T <= 2 while grid < SMs; T grows as M / SMs, ceil(M / 128) as M / 128, when grid = SMs).
+    const long ntiles = (M + BM - 1) / BM, half_tiles = (ntiles + 1) / 2;
+    const int grid = (int)(half_tiles < cmgan_num_sms() ? half_tiles : cmgan_num_sms());
     ffn_bwd_kernel<<<grid, NT, smem, (cudaStream_t)stream>>>(a);
-    if (cmgan_check_launch("ffn_bwd_kernel")) return -1;
-    // dLN = dh W1 on the tensor-core row GEMM (W1 image read transposed, already packed)
-    CmganGemmArgs gm;
-    memset(&gm, 0, sizeof(gm));
-    gm.A = dh_out; gm.lda = HID; gm.B = W1tp; gm.sb_k = C; gm.sb_n = 1; gm.C = dln; gm.ldc = C;
-    gm.M = (int)M; gm.N = C; gm.Cin = HID; gm.ntaps = 1; gm.mul_y = gm.mul_x = gm.div_y = gm.div_x = 1;
-    gm.epi = CMGAN_EPI_NONE; gm.pro = CMGAN_PRO_NONE; gm.alpha = 1.f; gm.precision = 1;
-    gm.ws = const_cast<float*>(W1tp); gm.ws_floats = (long long)C * HID; gm.b_packed = 1;
-    const int rc = cmgan_gemm_rows_tc_launch(&gm, (cudaStream_t)stream);
-    CMGAN_REQUIRE(rc <= 0, "cmgan_ffn_bwd: dLN shape not covered by the tensor-core GEMM");
-    if (rc) return -1;
-    return cmgan_ln_bwd(dln, C, x, ldx, stats, ln_g, M, dout, lddo, res2, res2 ? ldr2 : 0, dx, lddx, dgamma, dbeta, stream);
+    return cmgan_check_launch("ffn_bwd_kernel");
 }
