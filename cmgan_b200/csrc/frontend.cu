@@ -99,24 +99,25 @@ __global__ void pad_reflect_kernel(const float* __restrict__ x, long ldx, int L,
 // with its own head to Lw = ceil(L_b / 100) * 100, reflect-padded by 200 on both sides and scaled by c[b]; zero from Lw + 400 up to Lp.
 // Needs L_b >= Lw - L_b and Lw > 200 (checked on the host); the value of every element is the one cmgan_pad_reflect gives the padded
 // utterance alone.
-// FOLD (evaluation.py:25-34): every clip has L samples and lens is unused; clip b, wrap-padded to ceil(L / 100) * 100, is cut into k
-// segments of S = padded / k samples, and segment r becomes row b k + r, reflect-padded by 200 on each side (its own edges) and scaled by
-// c[b]: the rows signal.enhance feeds its DFT after the reshape, without the wrapped copy.  Needs S > 200 (checked on the host).
+// FOLD (evaluation.py:25-34): every clip has L samples and lens is unused; clip b, wrap-padded with its own head, is cut into segments of
+// S samples, and this launch fills k rows per clip: row b k + r is segment seg0 + r, reflect-padded by 200 on each side (its own edges) and
+// scaled by c[b] -- the rows signal.enhance feeds its DFT after the reshape, without the wrapped copy.  Needs S > 200 and a wrapped length
+// (seg0 + k) S <= 2 L (checked on the host).
 template <bool FOLD>
-__global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, int k,
+__global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, int k, int S, int seg0,
                                         const float* __restrict__ c, float* __restrict__ xp, int Lp) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int row = blockIdx.y;
     if (i >= Lp) return;
     const int b = FOLD ? row / k : row;
     const int Lb = FOLD ? L : clamp_len(__ldg(lens + b), L);
-    const int Lw = FOLD ? (L + HOP - 1) / HOP * HOP / k : (Lb + HOP - 1) / HOP * HOP;        // FOLD: the segment length S
+    const int Lw = FOLD ? S : (Lb + HOP - 1) / HOP * HOP;
     float v = 0.f;
     if (Lb > 0 && i < Lw + NFFT) {
         int j = i - NFFT / 2;
         if (j < 0) j = -j;
         if (j >= Lw) j = 2 * (Lw - 1) - j;
-        if (FOLD) j += (row - b * k) * Lw;            // segment r starts at sample r S of the wrapped clip
+        if (FOLD) j += (seg0 + row - b * k) * Lw;     // segment r starts at sample r S of the wrapped clip
         if (j >= Lb) j -= Lb;                         // wrap padding: sample Lb + k is sample k
         j = clamp_len(j, Lb - 1);                     // only reachable for lengths the host rejects
         v = __ldg(x + (long)b * ldx + j) * (c ? c[b] : 1.f);
@@ -617,13 +618,14 @@ int cmgan_rms_scale_frames(const float* x, long long ldx, int B, int L, const in
     return cmgan_check_launch("rms_scale_kernel");
 }
 
-int cmgan_pad_wrap_reflect_fold(const float* x, long long ldx, int B, int L, int k, const float* c, float* xp, int Lp, cudaStream_t st) {
-    const int S = (L + HOP - 1) / HOP * HOP / (k > 0 ? k : 1);
-    CMGAN_REQUIRE(x && xp && k > 0 && HOP % k == 0 && S > NFFT / 2 && Lp >= S + NFFT,
-                  "cmgan_pad_wrap_reflect_fold: need k | 100, S > 200 and Lp >= S + 400 (L=%d k=%d Lp=%d)", L, k, Lp);
+int cmgan_pad_wrap_reflect_fold(const float* x, long long ldx, int B, int L, int k, int S, int seg0, const float* c, float* xp, int Lp,
+                                cudaStream_t st) {
+    CMGAN_REQUIRE(x && xp && k > 0 && seg0 >= 0 && S > NFFT / 2 && Lp >= S + NFFT && (long long)(seg0 + k) * S <= 2LL * L,
+                  "cmgan_pad_wrap_reflect_fold: need S > 200, Lp >= S + 400 and (seg0 + k) S <= 2 L (L=%d k=%d S=%d seg0=%d Lp=%d)", L, k, S,
+                  seg0, Lp);
     if (B == 0) return 0;
     dim3 grid(cdiv(Lp, 256), B * k);
-    pad_wrap_reflect_kernel<true><<<grid, 256, 0, st>>>(x, ldx, L, nullptr, k, c, xp, Lp);
+    pad_wrap_reflect_kernel<true><<<grid, 256, 0, st>>>(x, ldx, L, nullptr, k, S, seg0, c, xp, Lp);
     return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 
@@ -668,7 +670,7 @@ CMGAN_API int cmgan_pad_wrap_reflect_ragged(const float* x, long long ldx, int B
                   "cmgan_pad_wrap_reflect_ragged: need Lp >= ceil(L / 100) * 100 + 400 (L=%d Lp=%d)", L, Lp);
     if (B == 0) return 0;
     dim3 grid(cdiv(Lp, 256), B);
-    pad_wrap_reflect_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, 1, c, xp, Lp);
+    pad_wrap_reflect_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, 1, 0, 0, c, xp, Lp);
     return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 

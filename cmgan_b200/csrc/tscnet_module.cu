@@ -547,81 +547,107 @@ void backward(Run& r, const Saved& sv, const float* x, long long sxb, long long 
 // ---- waveform in, waveform out (evaluation.py:21-53): the launch sequence of signal.enhance / enhance_ragged around forward()
 constexpr int NFFT = 400, HOP = 100;
 
-struct EnhanceGeom { int k, S, T, Lp, rows; };
+// k segments of S samples per clip, T frames per segment, Lp padded samples per row, rows = B k in all, run `pass` rows at a time
+struct EnhanceGeom { int k, S, T, Lp, rows, pass; };
 
-// evaluation.py:25-34: wrap padding to padded = ceil(L / 100) * 100; past cut_len the clip is folded into k segments of S = padded / k
-// samples, k = ceil(padded / cut_len) raised until it divides 100.  0, or -1 with the message set.
-int enhance_geom(int B, int L, int cut_len, bool ragged, EnhanceGeom& g, const char* who) {
+// The fold of a clip of L samples (signal.fold_geometry restates it): padded = ceil(L / 100) * 100, wrap-padded with the clip's own head.
+//   1. padded <= cut_len: one segment.
+//   2. the reference's rule (evaluation.py:30-34): k = ceil(padded / cut_len), raised until it divides 100, S = padded / k; each segment
+//      yields 100 floor(S / 100) samples, concatenated and cut to L.
+//   3. extend only, where rule 2 fails -- its loop never ends (k would pass 100) or its segments yield fewer than L samples (the reference's
+//      own length assertion fails): S_max = 100 floor(cut_len / 100) >= 300, k = ceil(padded / S_max), S = 100 ceil(padded / (100 k))
+//      <= S_max, wrap-padded to k S <= 2 L; the segments tile the clip without a gap.  The reference has no behaviour to match here.
+// 0, or -1 with the message set.  The 2^31 bound on rows * T is checked here for a single pass only (!extend).
+int enhance_geom(int B, int L, int cut_len, bool ragged, bool extend, EnhanceGeom& g, const char* who) {
     CMGAN_REQUIRE(B > 0, "%s: B must be positive (B=%d)", who, B);
     CMGAN_REQUIRE(L > NFFT / 2, "%s: L=%d samples; a clip needs more than the 200-sample reflect padding of the STFT", who, L);
     CMGAN_REQUIRE(cut_len > 0, "%s: cut_len must be positive (cut_len=%d)", who, cut_len);
     const long long padded = ((long long)L + HOP - 1) / HOP * HOP;
     CMGAN_REQUIRE(padded - L <= L, "%s: wrap padding L=%d to %lld is longer than the clip", who, L, padded);
-    long long k = 1;
+    long long k = 1, S = padded;
     if (padded > cut_len) {
         CMGAN_REQUIRE(!ragged, "%s: a ragged batch needs ceil(L / 100) * 100 <= cut_len (L=%d, cut_len=%d); longer clips take the uniform call, "
                       "which folds them", who, L, cut_len);
         k = (padded + cut_len - 1) / cut_len;
         while (k <= HOP && HOP % k != 0) ++k;
-        CMGAN_REQUIRE(k <= HOP, "%s: L=%d with cut_len=%d folds into more than 100 segments", who, L, cut_len);
+        if (k <= HOP) S = padded / k;
+        if (k > HOP || (extend && k * HOP * (S / HOP) < L)) {
+            CMGAN_REQUIRE(extend, "%s: L=%d with cut_len=%d folds into more than 100 segments", who, L, cut_len);
+            const long long smax = cut_len / HOP * HOP;
+            CMGAN_REQUIRE(smax >= 3 * HOP, "%s: cut_len=%d gives segments of at most %lld samples; a segment needs more than 200", who, cut_len, smax);
+            k = (padded + smax - 1) / smax;
+            S = (padded + HOP * k - 1) / (HOP * k) * HOP;
+            CMGAN_REQUIRE(k * S - L <= L, "%s: wrap padding L=%d to %lld segments of %lld samples is longer than the clip", who, L, k, S);
+        }
     }
     g.k = (int)k;
-    g.S = (int)(padded / k);
+    g.S = (int)S;
     CMGAN_REQUIRE(g.S > NFFT / 2, "%s: L=%d with cut_len=%d folds into %d segments of %d samples; a segment needs more than 200", who, L,
                   cut_len, g.k, g.S);
     g.T = g.S / HOP + 1;
     CMGAN_REQUIRE(k * HOP * (g.T - 1) >= L, "%s: L=%d with cut_len=%d folds into %d segments of %d samples, which yield only %lld samples", who,
                   L, cut_len, g.k, g.S, k * HOP * (g.T - 1));
-    const long long elems = (long long)B * k * g.T * NFEAT * CAT;
-    CMGAN_REQUIRE(elems < (1ll << 31), "%s: rows * T * 201 * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); split "
-                  "the batch", who, CAT, elems);
+    if (!extend) {
+        const long long elems = (long long)B * k * g.T * NFEAT * CAT;
+        CMGAN_REQUIRE(elems < (1ll << 31), "%s: rows * T * 201 * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer); "
+                      "split the batch", who, CAT, elems);
+    }
     g.rows = (int)(B * k);
+    g.pass = g.rows;
     g.Lp = (g.S + NFFT + HOP - 1) / HOP * HOP;
     return 0;
 }
 
+// The launch sequence of signal.enhance / enhance_ragged around forward(): the STFT tables and the RMS scales of the whole clips, then the
+// rows in passes of g.pass -- padding, DFT, compression, TSCNet, un-compression, inverse DFT, overlap-add into that pass's range of `out`.
+// Several passes only for one clip (B = 1): the segments share nothing but c.
 void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const int* lengths, const EnhanceGeom& g, float* out, long long ldo) {
-    const int T = g.T, rows = g.rows, F = NFEAT;
-    const long long MT = (long long)rows * T;
+    const int T = g.T, F = NFEAT;
     float* fwd = r.alloc((size_t)NFFT * 2 * F);
     float* inv = r.alloc((size_t)2 * F * NFFT);
     float* env = r.alloc((size_t)HOP * (T - 1));
     float* tail = r.alloc(HOP);
     float* c = r.alloc(B);
     int* tlen = r.alloc<int>(B);
-    float* X = r.alloc((size_t)MT * 2 * F);
-    float* fr = r.alloc((size_t)MT * F);
-    float* fi = r.alloc((size_t)MT * F);
+    float* X = r.alloc((size_t)g.pass * T * 2 * F);
+    float* fr = r.alloc((size_t)g.pass * T * F);
+    float* fi = r.alloc((size_t)g.pass * T * F);
     if (r.live()) r.ok(cmgan_stft_tables(fwd, inv, T, env, tail, r.st));
     if (r.live()) r.ok(lengths ? cmgan_rms_scale_frames(wav, ldw, B, L, lengths, c, tlen, r.st) : cmgan_rms_scale(wav, ldw, B, L, c, r.st));
     const size_t mark = r.top;
-    // ---- signal._stft_padded: wrap + reflect (+ fold) padding, framed DFT (exact fp32 FFMA), power compression
-    {
-        float* xp = r.alloc((size_t)rows * g.Lp);
-        float* S = r.alloc((size_t)MT * 2 * F);
+    const long long Lout = (long long)HOP * (T - 1);        // samples each segment yields
+    for (int s0 = 0; s0 < g.rows; s0 += g.pass) {
+        const int rows = std::min(g.pass, g.rows - s0), kp = rows / B;       // rows of this pass, segments per clip in it
+        const long long MT = (long long)rows * T;
+        // ---- signal._stft_padded: wrap + reflect (+ fold) padding, framed DFT (exact fp32 FFMA), power compression
+        {
+            float* xp = r.alloc((size_t)rows * g.Lp);
+            float* S = r.alloc((size_t)MT * 2 * F);
+            if (r.live())
+                r.ok(lengths ? cmgan_pad_wrap_reflect_ragged(wav, ldw, B, L, lengths, c, xp, g.Lp, r.st)
+                             : cmgan_pad_wrap_reflect_fold(wav, ldw, B, L, kp, g.S, s0, c, xp, g.Lp, r.st));
+            Gemm dft(xp, HOP, fwd, 0, 2 * F, 1, nullptr, S, 2 * F, MT, 2 * F, NFFT);
+            dft.conv(1, T, 1, g.Lp / HOP);
+            if (r.live()) r.ok(cmgan_gemm_rows_f32(&dft.a, r.st));          // precision 0 (memset by Gemm): the DFTs stay exact fp32
+            if (r.live()) r.ok(cmgan_compress(S, rows, T, X, r.st));
+            r.top = mark;
+        }
+        // ---- TSCNet.forward on (rows, 2, T, F) contiguous; a ragged batch passes its frame counts
+        r.frames = lengths ? tlen : nullptr;
+        forward(r, X, 2LL * T * F, (long long)T * F, F, 1, rows, T, F, fr, fi);
+        r.frames = nullptr;
+        r.top = mark;
+        // ---- signal.uncompress_istft_fwd: un-compression, inverse DFT (exact fp32 FFMA), overlap-add straight into `out`
+        float* U = r.alloc((size_t)MT * 2 * F);
+        float* frames = r.alloc((size_t)MT * NFFT);
+        if (r.live()) r.ok(cmgan_uncompress(fr, fi, (long long)T * F, F, 1, rows, T, U, r.st));
+        Gemm idft(U, 2 * F, inv, 0, NFFT, 1, nullptr, frames, NFFT, MT, NFFT, 2 * F);
+        if (r.live()) r.ok(cmgan_gemm_rows_f32(&idft.a, r.st));
         if (r.live())
-            r.ok(lengths ? cmgan_pad_wrap_reflect_ragged(wav, ldw, B, L, lengths, c, xp, g.Lp, r.st)
-                         : cmgan_pad_wrap_reflect_fold(wav, ldw, B, L, g.k, c, xp, g.Lp, r.st));
-        Gemm dft(xp, HOP, fwd, 0, 2 * F, 1, nullptr, S, 2 * F, MT, 2 * F, NFFT);
-        dft.conv(1, T, 1, g.Lp / HOP);
-        if (r.live()) r.ok(cmgan_gemm_rows_f32(&dft.a, r.st));          // precision 0 (memset by Gemm): the DFTs stay exact fp32
-        if (r.live()) r.ok(cmgan_compress(S, rows, T, X, r.st));
+            r.ok(lengths ? cmgan_ola_ragged_lengths(frames, B, T, tlen, lengths, L, env, tail, c, out, ldo, r.st)
+                         : cmgan_ola_fold(frames, rows, T, kp, env, c, out + s0 * Lout, ldo, (int)(L - s0 * Lout), r.st));
         r.top = mark;
     }
-    // ---- TSCNet.forward on (rows, 2, T, F) contiguous; a ragged batch passes its frame counts
-    r.frames = lengths ? tlen : nullptr;
-    forward(r, X, 2LL * T * F, (long long)T * F, F, 1, rows, T, F, fr, fi);
-    r.frames = nullptr;
-    r.top = mark;
-    // ---- signal.uncompress_istft_fwd: un-compression, inverse DFT (exact fp32 FFMA), overlap-add straight into `out`
-    float* U = r.alloc((size_t)MT * 2 * F);
-    float* frames = r.alloc((size_t)MT * NFFT);
-    if (r.live()) r.ok(cmgan_uncompress(fr, fi, (long long)T * F, F, 1, rows, T, U, r.st));
-    Gemm idft(U, 2 * F, inv, 0, NFFT, 1, nullptr, frames, NFFT, MT, NFFT, 2 * F);
-    if (r.live()) r.ok(cmgan_gemm_rows_f32(&idft.a, r.st));
-    if (r.live())
-        r.ok(lengths ? cmgan_ola_ragged_lengths(frames, B, T, tlen, lengths, L, env, tail, c, out, ldo, r.st)
-                     : cmgan_ola_fold(frames, rows, T, g.k, env, c, out, ldo, L, r.st));
 }
 
 }  // namespace
@@ -689,7 +715,7 @@ static long long enhance_bytes(int B, int L, const EnhanceGeom& g, int precision
 CMGAN_API long long cmgan_enhance_workspace_bytes(int B, int L, int cut_len, int precision) {
     if (precision != 0 && precision != 1) { cmgan_set_error("cmgan_enhance_workspace_bytes: precision must be 0 (fp32) or 1 (tf32)"); return -1; }
     EnhanceGeom g;
-    if (enhance_geom(B, L, cut_len, false, g, "cmgan_enhance_workspace_bytes") != 0) return -1;
+    if (enhance_geom(B, L, cut_len, false, false, g, "cmgan_enhance_workspace_bytes") != 0) return -1;
     return enhance_bytes(B, L, g, precision);
 }
 
@@ -699,7 +725,7 @@ CMGAN_API int cmgan_enhance(const float* params, const float* wav, long long ldw
     CMGAN_REQUIRE(precision == 0 || precision == 1, "cmgan_enhance: precision must be 0 (fp32) or 1 (tf32)");
     CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "cmgan_enhance: params must be 16-byte, workspace 256-byte aligned");
     EnhanceGeom g;
-    if (enhance_geom(B, L, cut_len, lengths != nullptr, g, "cmgan_enhance") != 0) return -1;
+    if (enhance_geom(B, L, cut_len, lengths != nullptr, false, g, "cmgan_enhance") != 0) return -1;
     CMGAN_REQUIRE(ldw >= L && ldo >= L, "cmgan_enhance: row strides must cover a clip (L=%d ldw=%lld ldo=%lld)", L, ldw, ldo);
     const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + (B - 1) * ldw + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + (B - 1) * ldo + L);
     CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "cmgan_enhance: wav and out overlap");
@@ -710,6 +736,51 @@ CMGAN_API int cmgan_enhance(const float* params, const float* wav, long long ldw
     r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
     r.st = (cudaStream_t)stream;
     enhance_walk(r, wav, ldw, B, L, lengths, g, out, ldo);
+    return r.rc;
+}
+
+// one clip of any length in passes of at most max_segments segments: the workspace is that of one pass of max_segments segments of the
+// longest S a fold can give at this cut_len (T_max = floor(cut_len / 100) + 1 frames), whatever L is
+static long long enhance_long_bytes(int cut_len, int max_segments, int precision, const char* who) {
+    CMGAN_REQUIRE(precision == 0 || precision == 1, "%s: precision must be 0 (fp32) or 1 (tf32)", who);
+    CMGAN_REQUIRE(cut_len >= 3 * HOP, "%s: cut_len=%d gives segments of at most %d samples; a segment needs more than 200", who, cut_len,
+                  cut_len / HOP * HOP);
+    CMGAN_REQUIRE(max_segments > 0, "%s: max_segments must be positive (max_segments=%d)", who, max_segments);
+    const int T = cut_len / HOP + 1;
+    const long long elems = (long long)max_segments * T * NFEAT * CAT;
+    CMGAN_REQUIRE(elems < (1ll << 31), "%s: max_segments * T * 201 * %d = %lld elements reach 2^31 (32-bit indexing of the encoder concat buffer; "
+                  "T = %d frames at cut_len=%d); lower max_segments", who, CAT, elems, T, cut_len);
+    const EnhanceGeom g{max_segments, cut_len, T, (cut_len + NFFT + HOP - 1) / HOP * HOP, max_segments, max_segments};
+    return enhance_bytes(1, cut_len, g, precision);
+}
+
+CMGAN_API long long cmgan_enhance_long_workspace_bytes(int cut_len, int max_segments, int precision) {
+    return enhance_long_bytes(cut_len, max_segments, precision, "cmgan_enhance_long_workspace_bytes");
+}
+
+CMGAN_API int cmgan_enhance_long(const float* params, const float* wav, int L, int cut_len, int max_segments, float* out, void* workspace,
+                                 long long workspace_bytes, int precision, void* stream) {
+    const char* who = "cmgan_enhance_long";
+    CMGAN_REQUIRE(params && wav && out && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    CMGAN_REQUIRE(L <= (1 << 30), "%s: L=%d samples; at most 2^30 (18.6 hours at 16 kHz) keeps every sample index in 32 bits", who, L);
+    const long long need = enhance_long_bytes(cut_len, max_segments, precision, who);
+    if (need < 0) return -1;
+    EnhanceGeom g;
+    if (enhance_geom(1, L, cut_len, false, true, g, who) != 0) return -1;
+    const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + L);
+    CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "%s: wav and out overlap", who);
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    g.pass = std::min(max_segments, g.k);
+    EnhanceGeom first = g;          // every pass starts from the same mark, and the first one is the largest
+    first.rows = g.pass;
+    const long long run = enhance_bytes(1, L, first, precision);
+    CMGAN_REQUIRE(run <= need, "%s: internal error: L=%d needs %lld workspace bytes, more than the query's %lld", who, L, run, need);
+    cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
+    Run r;
+    r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
+    r.st = (cudaStream_t)stream; r.who = who;
+    enhance_walk(r, wav, L, 1, L, nullptr, g, out, L);
     return r.rc;
 }
 

@@ -25,7 +25,7 @@ import torch
 from . import signal
 
 SR = 16000
-MAX_ELEMENTS = 2 ** 31          # the widest activation buffer (B * T * 201 * 320 floats) is indexed with 32-bit element counts
+MAX_ELEMENTS = signal.MAX_ELEMENTS
 
 
 def read_wav(path: str) -> Tuple[torch.Tensor, int]:

@@ -243,6 +243,9 @@ class TSCNet(nn.Module):
             raise RuntimeError("cmgan_b200.TSCNet runs on CUDA only (no CPU fallback)")
         if x.dtype != torch.float32:
             raise RuntimeError("cmgan_b200.TSCNet expects float32 input")
+        if x.dim() == 4 and x.shape[0] * x.shape[2] * x.shape[3] * 320 >= 2 ** 31:
+            raise ValueError(f"B * T * F * 320 = {x.shape[0] * x.shape[2] * x.shape[3] * 320} elements reach 2^31 (32-bit indexing of the "
+                             "encoder concat buffer); split the batch")
         if frames is not None:
             return self._forward_ragged(x, frames)
         if self.training:

@@ -2,7 +2,8 @@
 
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
-out.  ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
+out, and ``cmgan_enhance_long`` runs one clip of any length through a fixed-size workspace, a few folded segments at a time.
+``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
 parameter and input gradients.  ``cmgan_disc_fwd`` / ``cmgan_disc_bwd`` are the same pair for the metric discriminator (ref: discriminator.py:29-64),
 with the spectral-norm power iteration, parameter gradients through the spectral norm and input gradients.  ``cmgan_gen_wave_fwd`` /
 ``cmgan_gen_wave_bwd`` wrap the TSCNet pair in the STFT front end, the inverse STFT and the spectral and time-domain losses (ref:
@@ -15,6 +16,7 @@ from typing import Dict, List, Tuple
 
 import torch
 
+from . import signal
 from ._lib import lib
 
 
@@ -96,6 +98,41 @@ def enhance(flat: torch.Tensor, wav: torch.Tensor, lengths=None, cut_len: int = 
         assert lens.numel() == B, f"lengths has {lens.numel()} entries for a batch of {B}"
     lib().call("cmgan_enhance", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), cut_len,
                out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    return out
+
+
+def _long_segments(cut_len: int, max_segments, k: int = None) -> int:
+    """max_segments=None: the most segments of the longest fold at this cut_len (T_max = cut_len // 100 + 1 frames) one pass takes, at most k"""
+    if max_segments is not None:
+        return max_segments
+    n = signal.max_pass_rows(cut_len // signal.HOP + 1)
+    return n if k is None else min(n, k)
+
+
+def enhance_long_workspace_bytes(cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1) -> int:
+    """workspace of ``cmgan_enhance_long``: the same for every clip length"""
+    n = lib().cdll.cmgan_enhance_long_workspace_bytes(cut_len, _long_segments(cut_len, max_segments), precision)
+    if n < 0:
+        raise RuntimeError(lib().cdll.cmgan_last_error().decode())
+    return n
+
+
+def enhance_long(flat: torch.Tensor, wav: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1,
+                 workspace: torch.Tensor = None, out: torch.Tensor = None) -> torch.Tensor:
+    """``cmgan_enhance_long``: one noisy clip of any length (1-D, contiguous, on the GPU) -> the enhanced clip in ``out`` (same length), which is
+    returned.  The fold's segments (``signal.fold_geometry``) run ``max_segments`` at a time through one workspace whose size does not depend
+    on the length; None = as many as one pass of the longest segments takes (13 at cut_len = 16 s), at most the clip's segment count."""
+    assert wav.is_cuda and flat.is_cuda and wav.dtype == torch.float32 and wav.dim() == 1 and wav.is_contiguous()
+    L = wav.numel()
+    k, _ = signal.fold_geometry(L, cut_len)
+    n = _long_segments(cut_len, max_segments, k)
+    if workspace is None:
+        workspace = torch.empty(enhance_long_workspace_bytes(cut_len, n, precision), dtype=torch.uint8, device=wav.device)
+    if out is None:
+        out = torch.empty(L, device=wav.device)
+    assert out.is_cuda and out.dtype == torch.float32 and out.dim() == 1 and out.numel() >= L and out.is_contiguous()
+    lib().call("cmgan_enhance_long", flat.data_ptr(), wav.data_ptr(), L, cut_len, n, out.data_ptr(), workspace.data_ptr(), workspace.numel(),
+               precision, torch.cuda.current_stream().cuda_stream)
     return out
 
 

@@ -12,6 +12,7 @@ from typing import Dict, List, Sequence, Tuple
 
 import torch
 
+from . import ops
 from .ops import call, gemm
 
 N_FFT, HOP, NF = 400, 100, 201
@@ -263,27 +264,99 @@ def enhance_batch(model, noisy: torch.Tensor) -> torch.Tensor:
     return uncompress_istft(fr, fi, c)[:, :length]
 
 
+def fold_geometry(length: int, cut_len: int = 16000 * 16) -> Tuple[int, int]:
+    """(k, S): how ``enhance`` cuts a clip of ``length`` samples into k segments of S samples after wrap padding it with its own head to k S
+    (the C entries' ``enhance_geom``).  padded = ceil(length / 100) * 100.
+    1. padded <= cut_len: one segment of padded samples.
+    2. the reference's rule (evaluation.py:30-34), where it ends: k = ceil(padded / cut_len) raised until it divides 100 (k <= 100),
+       S = padded / k; each segment yields 100 floor(S / 100) samples, concatenated and cut to ``length``.
+    3. where rule 2 fails -- its loop never ends (padded > 100 cut_len) or its segments yield fewer than ``length`` samples (the reference's
+       own length assertion fails) -- an extension with no reference behaviour to match: S_max = 100 floor(cut_len / 100) >= 300,
+       k = ceil(padded / S_max), S = 100 ceil(padded / (100 k)) <= S_max; the segments tile the clip wrap-padded to k S <= 2 length.
+    Raises ValueError when no fold exists: a segment of 200 samples or fewer, or one that yields fewer than ``length`` samples."""
+    padded = -(-length // HOP) * HOP
+    if length <= N_FFT // 2 or padded - length > length:
+        raise ValueError(f"a clip of {length} samples is too short for the wrap padding to {padded} and the 200-sample reflect padding")
+    k, S = 1, padded
+    if padded > cut_len:
+        k = -(-padded // cut_len)
+        while k <= HOP and HOP % k != 0:
+            k += 1
+        if k <= HOP:
+            S = padded // k
+        if k > HOP or k * HOP * (S // HOP) < length:
+            smax = cut_len // HOP * HOP
+            if smax < 3 * HOP:
+                raise ValueError(f"cut_len = {cut_len} gives segments of at most {smax} samples; a segment needs more than 200")
+            k = -(-padded // smax)
+            S = -(-padded // (HOP * k)) * HOP
+            if k * S - length > length:
+                raise ValueError(f"a clip of {length} samples is too short for the wrap padding to {k} segments of {S} samples")
+    if S <= N_FFT // 2 or k * HOP * (S // HOP) < length:
+        raise ValueError(f"a clip of {length} samples with cut_len = {cut_len} folds into {k} segments of {S} samples, which cannot hold it")
+    return k, S
+
+
+MAX_ELEMENTS = 2 ** 31          # the encoder's concat buffer (rows * T * 201 * 320 floats) is indexed with 32-bit element counts
+
+
+def max_pass_rows(T: int) -> int:
+    """the most rows of T frames one TSCNet forward takes: rows * T * 201 * 320 < 2^31"""
+    return (MAX_ELEMENTS - 1) // (T * NF * 320)
+
+
+# Peak device memory of one pass of the Python walk (stft_compress, TSCNet.forward, uncompress_istft) per frame of a row, by precision
+# (ops.PRECISION).  Measured on an H100 80GB HBM3 at rows 1 and 2, T = 601, 1201 and 2401: 8.85-8.91 MB in fp32, 5.11-5.15 MB in tf32,
+# linear in rows * T; rounded up here.
+PASS_BYTES_PER_FRAME = {0: 9.0e6, 1: 5.2e6}
+
+
+def default_pass_rows(k: int, T: int, device) -> int:
+    """rows per pass of ``enhance`` when the caller gives none.  All k when they fit under 2^31: the single batch of the reference's fold,
+    what ``enhance`` has always run for such clips.  Otherwise as many as the 2^31 bound and 90 % of the device memory that is free now
+    (including what torch's allocator holds unused) take, at least 1."""
+    if k <= max_pass_rows(T):
+        return k
+    free, _ = torch.cuda.mem_get_info(device)
+    free += torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+    fit = int(0.9 * free // (PASS_BYTES_PER_FRAME[ops.PRECISION] * T))
+    return max(1, min(k, max_pass_rows(T), fit))
+
+
 @torch.no_grad()
-def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16) -> torch.Tensor:
-    """evaluation.enhance_one_track between load and save (ref: evaluation.py:21-53) on the GPU: (1, L) -> (L,)."""
+def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None) -> torch.Tensor:
+    """evaluation.enhance_one_track between load and save (ref: evaluation.py:21-53) on the GPU: (1, L) -> (L,), for a clip of any length.
+    The clip is folded as ``fold_geometry`` says; its k segments run through the model ``max_segments`` at a time, all scaled by the whole
+    clip's RMS.  Segments share nothing else, so every pass computes what the single-batch fold computes for its rows.  The default
+    (``default_pass_rows``) is one pass of all k rows, the reference's batch, when they fit under 2^31, and otherwise as many rows as fit in
+    the free device memory (about 5.2 MB per frame in tf32, 9 MB in fp32: 5 rows of 16 s segments in tf32 on an idle 80 GB H100).
+    ``module_abi.enhance_long`` runs the same passes in a fixed workspace (19.8 GB for 13 rows at cut_len = 16 s, tf32)."""
     assert noisy.dim() == 2 and noisy.shape[0] == 1
+    if max_segments is not None and max_segments <= 0:
+        raise ValueError(f"max_segments must be positive (max_segments={max_segments})")
     noisy = noisy.contiguous()
     length = noisy.size(-1)
+    k, S = fold_geometry(length, cut_len)
     c = rms_scale(noisy)
-    padded_len = int(math.ceil(length / 100)) * 100
-    if padded_len != length:            # wrap padding with the signal's own head (evaluation.py:25-29)
-        noisy = torch.cat([noisy, noisy[:, :padded_len - length]], dim=-1)
-    batch = 1
-    if padded_len > cut_len:            # fold long files into the batch (evaluation.py:30-34)
-        batch = int(math.ceil(padded_len / cut_len))
-        while 100 % batch != 0:
-            batch += 1
-        noisy = noisy.reshape(batch, -1)
-    cb = c.expand(batch).contiguous() if batch > 1 else c
-    spec = stft_compress(noisy, cb).permute(0, 1, 3, 2)
-    fr, fi = model(spec)
-    audio = uncompress_istft(fr, fi, cb)
-    return audio.reshape(-1)[:length]
+    if k * S != length:                 # wrap padding with the signal's own head (evaluation.py:25-29)
+        noisy = torch.cat([noisy, noisy[:, :k * S - length]], dim=-1)
+    rows = noisy.reshape(k, S)          # fold long files into the batch (evaluation.py:30-34)
+    T = S // HOP + 1
+    n = min(k, max_segments) if max_segments is not None else default_pass_rows(k, T, noisy.device)
+    out = None if n == k else torch.empty(length, device=noisy.device)
+    seg_out = HOP * (T - 1)
+    for s0 in range(0, k, n):
+        m = min(n, k - s0)
+        cb = c.expand(m).contiguous() if m > 1 else c
+        spec = stft_compress(rows[s0:s0 + m], cb).permute(0, 1, 3, 2)
+        fr, fi = model(spec)
+        audio = uncompress_istft(fr, fi, cb).reshape(-1)
+        if out is None:
+            return audio[:length]
+        o0 = s0 * seg_out
+        cnt = min(length - o0, m * seg_out)
+        out[o0:o0 + cnt] = audio[:cnt]
+    return out
 
 
 def ragged_padded_length(length: int, cut_len: int = 16000 * 16) -> int:

@@ -1,8 +1,10 @@
 /* Speech enhancement from a non-Python host (plain C99): one noisy mono clip in, the enhanced clip out, through the waveform-level entry
- * cmgan_enhance of libcmgan_b200.so (evaluation.py:21-53 as one call).
+ * cmgan_enhance of libcmgan_b200.so (evaluation.py:21-53 as one call), or through cmgan_enhance_long, which runs a clip of any length a few
+ * folded segments at a time in a workspace whose size does not depend on the length.
  *   Build:  gcc -std=c99 -Iinclude examples/c_enhance.c -o c_enhance -Lcmgan_b200 -lcmgan_b200 -Wl,-rpath,$PWD/cmgan_b200
  *           (add -DWITH_CUDA -I/usr/local/cuda/include -L/usr/local/cuda/lib64 -lcudart to enhance a clip).
- *   Run:    c_enhance [params.f32 noisy.f32 enhanced.f32 [precision [cut_len]]]
+ *   Run:    c_enhance [params.f32 noisy.f32 enhanced.f32 [precision [cut_len [max_segments]]]]
+ *           (max_segments > 0 switches to cmgan_enhance_long with passes of at most that many segments)
  * params.f32 is a raw little-endian float32 dump of the parameter block (cmgan_b200.module_abi.pack_params(...).cpu().numpy().tofile(path));
  * noisy.f32 / enhanced.f32 are raw little-endian float32 samples at 16 kHz (the reference reads 16-bit wav files and divides by 32768).
  * Without WITH_CUDA only the host-side workspace queries and argument checks run (no GPU needed). */
@@ -33,9 +35,20 @@ int main(int argc, char** argv) {
     printf("rejected L=1700 cut_len=1000: %s\n", cmgan_last_error());
     if (cmgan_enhance(NULL, NULL, 0, 1, 16000, NULL, 16000 * 16, NULL, 0, NULL, 0, 1, NULL) == 0) { fprintf(stderr, "null pointers must be rejected\n"); return 1; }
     printf("rejected call: %s\n", cmgan_last_error());
+    /* the long entry's workspace depends on cut_len, max_segments and precision only; at 16 s, 13 segments are the most one pass takes */
+    const int segs[4] = {1, 4, 8, 13};
+    for (int i = 0; i < 4; ++i) {
+        const int m = segs[i];
+        const long long ws = cmgan_enhance_long_workspace_bytes(16000 * 16, m, 1);
+        if (ws < 0) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
+        printf("workspace long cut_len=%d max_segments=%d tf32: %lld bytes\n", 16000 * 16, m, ws);
+    }
+    if (cmgan_enhance_long_workspace_bytes(16000 * 16, 14, 1) >= 0) { fprintf(stderr, "14 segments of 16 s must be rejected\n"); return 1; }
+    printf("rejected max_segments=14: %s\n", cmgan_last_error());
 #ifdef WITH_CUDA
     if (argc > 3) {
         const int precision = argc > 4 ? atoi(argv[4]) : 1, cut_len = argc > 5 ? atoi(argv[5]) : 16000 * 16;
+        const int max_segments = argc > 6 ? atoi(argv[6]) : 0;
         const long long total = cmgan_tscnet_param_floats();
         float* hp = (float*)malloc((size_t)total * 4);
         FILE* f = fopen(argv[1], "rb");
@@ -49,7 +62,8 @@ int main(int argc, char** argv) {
         float* hx = (float*)malloc((size_t)L * 4);
         if (L <= 0 || fread(hx, 4, (size_t)L, f) != (size_t)L) { fprintf(stderr, "cannot read %s\n", argv[2]); return 1; }
         fclose(f);
-        const long long ws = cmgan_enhance_workspace_bytes(1, L, cut_len, precision);
+        const long long ws = max_segments > 0 ? cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision)
+                                              : cmgan_enhance_workspace_bytes(1, L, cut_len, precision);
         if (ws < 0) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
         float *params, *x, *y;
         void* wsp;
@@ -60,12 +74,14 @@ int main(int argc, char** argv) {
         }
         cudaMemcpy(params, hp, (size_t)total * 4, cudaMemcpyHostToDevice);
         cudaMemcpy(x, hx, (size_t)L * 4, cudaMemcpyHostToDevice);
-        if (cmgan_enhance(params, x, L, 1, L, NULL, cut_len, y, L, wsp, ws, precision, 0)) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
+        const int rc = max_segments > 0 ? cmgan_enhance_long(params, x, L, cut_len, max_segments, y, wsp, ws, precision, 0)
+                                        : cmgan_enhance(params, x, L, 1, L, NULL, cut_len, y, L, wsp, ws, precision, 0);
+        if (rc) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
         if (cudaMemcpy(hx, y, (size_t)L * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { fprintf(stderr, "device error\n"); return 1; }
         f = fopen(argv[3], "wb");
         if (!f || fwrite(hx, 4, (size_t)L, f) != (size_t)L) { fprintf(stderr, "cannot write %s\n", argv[3]); return 1; }
         fclose(f);
-        printf("enhanced %d samples (precision %d, workspace %lld bytes)\n", L, precision, ws);
+        printf("enhanced %d samples (precision %d, workspace %lld bytes%s)\n", L, precision, ws, max_segments > 0 ? ", long entry" : "");
         cudaFree(params); cudaFree(x); cudaFree(y); cudaFree(wsp);
         free(hp); free(hx);
     }

@@ -250,6 +250,26 @@ int cmgan_cut_batch(const float* corpus, const long long* offsets, const int* le
 long long cmgan_enhance_workspace_bytes(int B, int L, int cut_len, int precision);
 int cmgan_enhance(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int cut_len, float* out, long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream);
 
+/* ---- module level, waveform in / waveform out for ONE clip of any length in bounded memory: cmgan_enhance's fold, run a few segments at a time.
+ * wav, out: L samples on the device; only wav[:L] is read and only out[:L] written; the ranges may not overlap.  The RMS scale is computed once
+ * over the whole clip (the kernel and summation order of cmgan_enhance), then the k segments of the fold run in passes of at most max_segments
+ * rows through one workspace: padding, STFT, compression, TSCNet.forward, un-compression, inverse STFT and overlap-add into the pass's range
+ * of out.  Segments share nothing but the scale, so a pass computes exactly what the single-batch fold computes for its rows.
+ *   Fold: padded = ceil(L / 100) * 100.  padded <= cut_len: one segment.  Otherwise the reference's rule (k = ceil(padded / cut_len) raised
+ *   until it divides 100, S = padded / k), as cmgan_enhance, wherever it gives a fold: k <= 100 and k 100 floor(S / 100) >= L samples out.
+ *   Where it does not -- padded > 100 cut_len, where the reference loops forever, or segments that yield fewer than L samples (any k that does
+ *   not divide padded / 100; the reference's own length assertion fails and cmgan_enhance rejects the clip) -- an extension with no reference
+ *   behaviour to match: S_max = 100 floor(cut_len / 100), k = ceil(padded / S_max), S = 100 ceil(padded / (100 k)); the clip is wrap-padded
+ *   with its own head to k S <= 2 L and the segment outputs tile it without a gap.
+ * cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision) depends on neither L nor the clip: one buffer serves every length.
+ * Both return -1 (message in cmgan_last_error; nothing launched) for null or misaligned pointers (params 16-byte, workspace 256-byte),
+ * L <= 200 or L > 2^30, cut_len < 300 (no segment of more than 200 samples), max_segments <= 0, max_segments * T_max * 201 * 320 >= 2^31
+ * (T_max = floor(cut_len / 100) + 1; 13 segments at cut_len = 16 s), overlapping wav / out, precision not 0 / 1, a workspace smaller than
+ * the query, or a fold into segments of 200 samples or fewer (small cut_len only).  Allocates nothing,
+ * never synchronises, CUDA-graph capturable. */
+long long cmgan_enhance_long_workspace_bytes(int cut_len, int max_segments, int precision);
+int cmgan_enhance_long(const float* params, const float* wav, int L, int cut_len, int max_segments, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
