@@ -23,6 +23,11 @@ __device__ double block_sum_d(double v, double* sm) {
     return t;
 }
 
+// numpy's minimum / maximum: NaN when either operand is NaN (CUDA's fmin / fmax return the other operand).  The reference clips and
+// floors with NaN-propagating operations, so a silent or non-finite processed signal scores NaN there and must score NaN here too.
+__device__ __forceinline__ double np_min(double a, double b) { return (isnan(a) || isnan(b)) ? a + b : fmin(a, b); }
+__device__ __forceinline__ double np_max(double a, double b) { return (isnan(a) || isnan(b)) ? a + b : fmax(a, b); }
+
 // ---- segmental SNR: one block per frame; out[0] += clipped frame value / nfr
 __global__ void ssnr_kernel(const double* __restrict__ c, const double* __restrict__ p, int W, int skip, int nfr, double* __restrict__ out) {
     __shared__ double sm[32];
@@ -40,7 +45,7 @@ __global__ void ssnr_kernel(const double* __restrict__ c, const double* __restri
     if (threadIdx.x == 0) {
         const double eps = 2.220446049250313e-16;
         double v = 10.0 * log10(se / (ne + eps) + eps);
-        v = fmin(fmax(v, -10.0), 35.0);
+        v = np_min(np_max(v, -10.0), 35.0);
         atomicAdd(out, v / (double)nfr);
     }
 }
@@ -80,19 +85,20 @@ __global__ void frame_level_kernel(const double* __restrict__ x, long len, int n
     if (threadIdx.x == 0) lev[j] = 20.0 * log10(sqrt(e) / 16.0);       // / sqrt(N), N = 256
 }
 
-// one block: max level, keep mask, compaction map.  kept[c] = source frame of the c-th kept frame; cnt[0] = number kept
+// one block: max level, keep mask, compaction map.  kept[c] = source frame of the c-th kept frame; cnt[0] = number kept.  Fully silent
+// frames (level -inf) lie below the -1e300 start and are dropped; a NaN level makes the maximum NaN (np.max) and then no frame is kept.
 __global__ void silent_mask_kernel(const double* __restrict__ lev, int nframes, double dyn, int* __restrict__ kept, int* __restrict__ cnt) {
     __shared__ double smx[32];
     __shared__ int soff;
     double m = -1e300;
-    for (int j = threadIdx.x; j < nframes; j += blockDim.x) m = fmax(m, lev[j]);
+    for (int j = threadIdx.x; j < nframes; j += blockDim.x) m = np_max(m, lev[j]);
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    for (int o = 16; o > 0; o >>= 1) m = np_max(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) smx[threadIdx.x >> 5] = m;
     if (threadIdx.x == 0) soff = 0;
     __syncthreads();
     m = smx[0];
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, smx[w]);
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = np_max(m, smx[w]);
     // ordered compaction, 1024 frames per pass (one thread per frame, warp ballots + a serial pass over the 32 warp totals)
     __shared__ int wtot[32];
     for (int base = 0; base < nframes; base += blockDim.x) {
@@ -186,7 +192,8 @@ __global__ void stoi_segment_kernel(const double* __restrict__ X, const double* 
         const double c = 5.623413251903491;          // 10^(15/20)
         double yp[NSEG];
         double mx = 0.0, my = 0.0;
-        for (int n = 0; n < NSEG; ++n) { yp[n] = fmin(yr[n] * alpha, xr[n] + xr[n] * c); mx += xr[n]; my += yp[n]; }
+        // a processed band that is zero over the segment gives alpha = inf and 0 * inf = NaN: the segment, like the reference's, is NaN
+        for (int n = 0; n < NSEG; ++n) { yp[n] = np_min(yr[n] * alpha, xr[n] + xr[n] * c); mx += xr[n]; my += yp[n]; }
         mx /= NSEG; my /= NSEG;
         double nx = 0.0, ny = 0.0, dot = 0.0;
         for (int n = 0; n < NSEG; ++n) { const double a = xr[n] - mx, b = yp[n] - my; nx += a * a; ny += b * b; dot += a * b; }
@@ -328,7 +335,7 @@ __global__ void wss_kernel(const double* __restrict__ c, const double* __restric
             const double* spec = tid < WSS_NB ? sc : sp;
             double acc = 0.0;
             for (int j = 0; j < half; ++j) acc += filt[b * half + j] * spec[j];
-            const double v = 10.0 * log10(fmax(acc, 1e-10));
+            const double v = 10.0 * log10(np_max(acc, 1e-10));
             if (tid < WSS_NB) ec[b] = v; else ep[b] = v;
         }
     } else {
@@ -339,7 +346,7 @@ __global__ void wss_kernel(const double* __restrict__ c, const double* __restric
             for (int j = lane; j < half; j += 32) acc += filt[b * half + j] * spec[j];
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-            const double v = 10.0 * log10(fmax(acc, 1e-10));
+            const double v = 10.0 * log10(np_max(acc, 1e-10));
             if (lane == 0) { if (job < WSS_NB) ec[b] = v; else ep[b] = v; }
         }
     }
@@ -348,7 +355,7 @@ __global__ void wss_kernel(const double* __restrict__ c, const double* __restric
         double csl[WSS_NB - 1], psl[WSS_NB - 1], cpk[WSS_NB - 1], ppk[WSS_NB - 1];
         double cmax = ec[0], pmax = ep[0];
         for (int i = 0; i < WSS_NB - 1; ++i) { csl[i] = ec[i + 1] - ec[i]; psl[i] = ep[i + 1] - ep[i]; }
-        for (int i = 1; i < WSS_NB; ++i) { cmax = fmax(cmax, ec[i]); pmax = fmax(pmax, ep[i]); }
+        for (int i = 1; i < WSS_NB; ++i) { cmax = np_max(cmax, ec[i]); pmax = np_max(pmax, ep[i]); }
         wss_peaks(ec, csl, cpk);
         wss_peaks(ep, psl, ppk);
         double num = 0.0, den = 0.0;
@@ -365,8 +372,8 @@ __global__ void wss_kernel(const double* __restrict__ c, const double* __restric
 
 }  // namespace
 
-// mean segmental SNR (dB) of `proc` against `clean` (float64, L samples): out[0] must be zero on entry.  nfr = int(L / skip - W / skip) is the
-// caller's (it is a host-side float expression in the reference).
+// mean segmental SNR (dB) of `proc` against `clean` (float64, L samples), added to out[0]: zero it on entry for the mean itself.  nfr =
+// int(L / skip - W / skip) is the caller's (it is a host-side float expression in the reference); nfr = 0 writes nothing.
 CMGAN_API int cmgan_ssnr_f64(const double* clean, const double* proc, long long L, int W, int skip, int nfr, double* out, void* stream) {
     CMGAN_REQUIRE(clean && proc && out && W > 0 && skip > 0, "cmgan_ssnr_f64: bad arguments");
     CMGAN_REQUIRE(nfr >= 0 && (long long)(nfr - 1) * skip + W <= L, "cmgan_ssnr_f64: frames exceed the signal");
