@@ -1,12 +1,13 @@
 #!/usr/bin/env python
 """Per-call times of the fused feed-forward kernels at the bench shape (B = 16 x 2 s: M = 16 x 321 x 101 rows, C = 64, hidden 256).
 
-    python tools/bench_ffn.py [--M 518736] [--iters 50] [--warmup 5]
+    python tools/bench_ffn.py [--M 518736] [--iters 50] [--warmup 5] [--save DIR]
 
 Times cmgan_ffn_fwd and cmgan_ffn_bwd (training dropout, res2 on, as the second feed-forward of a conformer block calls it) with CUDA
 events over --iters back-to-back calls after a warm-up, and prints microseconds per call with the algorithmic HBM bytes and FLOPs
 (computed from the shapes below), the achieved GB/s and TFLOP/s, and the fraction of the floor set by the H100 SXM data-sheet peaks.
-The card name, power limit and SM clock are printed with the numbers.
+The card name, power limit and SM clock are printed with the numbers.  --save DIR first runs each call once on the same seeded inputs and
+writes every output (out, dx, a, dh, xn, stats, dgamma, dbeta) to DIR/<name>.pt, so that two builds can be compared bit for bit.
 """
 import argparse
 import json
@@ -64,6 +65,7 @@ def main():
     ap.add_argument("--M", type=int, default=16 * 321 * 101)
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--save", metavar="DIR", default=None, help="write the outputs of one call of each kernel to DIR/<name>.pt")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_ffn: no CUDA device")
@@ -91,6 +93,15 @@ def main():
 
     def bwd():
         call("cmgan_ffn_bwd", x, C, dz, C, dout, C, res2, C, M, g, b, W1p, b1, W2tp, W1tp, 1, thr, inv, None, dx, C, a, dh, xn, dg, db, ws)
+
+    if args.save:
+        fwd()
+        bwd()
+        torch.cuda.synchronize()
+        os.makedirs(args.save, exist_ok=True)
+        outs = {"out": out, "dx": dx, "a": a, "dh": dh, "xn": xn, "stats": ws[C * M:], "dgamma": dg, "dbeta": db}
+        for name, t in outs.items():
+            torch.save(t.cpu(), os.path.join(args.save, name + ".pt"))
 
     res = {"M": M, "iters": args.iters, **card(), "kernels": {}}
     tr = traffic(M)
