@@ -6,6 +6,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "resample.cuh"
 #include "../../include/cmgan_b200.h"
 
 namespace {
@@ -48,20 +49,6 @@ __global__ void ssnr_kernel(const double* __restrict__ c, const double* __restri
         v = np_min(np_max(v, -10.0), 35.0);
         atomicAdd(out, v / (double)nfr);
     }
-}
-
-// ---- polyphase resampling 16 kHz -> 10 kHz (scipy.signal.resample_poly(x, 10000, 16000): up 5, down 8, 161-tap Kaiser(5) low-pass h, already
-// multiplied by up):  y[n] = sum_i x[i] h[8 n + 80 - 5 i]
-__global__ void resample_kernel(const double* __restrict__ x, long n_in, const double* __restrict__ h, double* __restrict__ y, long n_out) {
-    const long n = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= n_out) return;
-    const long t = 8 * n + 80;
-    long i_hi = t / 5, i_lo = (t - 160 + 4) / 5;
-    if (t - 160 < 0) i_lo = 0;
-    if (i_hi > n_in - 1) i_hi = n_in - 1;
-    double acc = 0.0;
-    for (long i = i_lo; i <= i_hi; ++i) acc += x[i] * h[t - 5 * i];
-    y[n] = acc;
 }
 
 __device__ __forceinline__ double hann_inner(int i) {      // scipy.signal.windows.hann(N + 2)[1 : N + 1], N = 256 (symmetric window of 258 points)
@@ -400,8 +387,9 @@ CMGAN_API int cmgan_stoi_f64(const double* clean, const double* proc, long long 
     double* x10 = scratch; double* y10 = x10 + n10 + NF; double* xs = y10 + n10 + NF; double* ys = xs + n10 + NF;
     double* lev = ys + n10 + NF; double* X = lev + nframes + 1; double* Y = X + (long)NBAND * nframes;
     int* kept = reinterpret_cast<int*>(Y + (long)NBAND * nframes); int* cnt = kept + nframes + 1;
-    resample_kernel<<<cdiv(n10, 256), 256, 0, st>>>(clean, L, h, x10, n10);
-    resample_kernel<<<cdiv(n10, 256), 256, 0, st>>>(proc, L, h, y10, n10);
+    // scipy.signal.resample_poly(x, 10000, 16000): up 5, down 8, the 161 taps of h (already x 5)
+    if (resample::launch<double>(clean, L, 1, L, nullptr, 5, 8, 80, h, x10, n10, n10, nullptr, nullptr, st) != 0) return -1;
+    if (resample::launch<double>(proc, L, 1, L, nullptr, 5, 8, 80, h, y10, n10, n10, nullptr, nullptr, st) != 0) return -1;
     frame_level_kernel<<<nframes, 128, 0, st>>>(x10, n10, nframes, lev);
     silent_mask_kernel<<<1, 1024, 0, st>>>(lev, nframes, 40.0, kept, cnt);
     compact_kernel<<<cdiv(max_out, 256), 256, 0, st>>>(x10, y10, kept, cnt, xs, ys, max_out);

@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "frontend.cuh"
 #include "module_walk.cuh"
+#include "resample.cuh"
 #include "../../include/cmgan_b200.h"
 
 namespace {
@@ -782,6 +783,126 @@ CMGAN_API int cmgan_enhance_long(const float* params, const float* wav, int L, i
     r.st = (cudaStream_t)stream; r.who = who;
     enhance_walk(r, wav, L, 1, L, nullptr, g, out, L);
     return r.rc;
+}
+
+// ==================================================================================== any sample rate: resample, the 16 kHz walk, resample back
+// The model runs at 16 kHz.  At another rate sr the entries resample the clips to 16 kHz into the workspace, run cmgan_enhance /
+// cmgan_enhance_long there on the rest of the workspace, and resample the 16 kHz result back into the caller's out, cut to each clip's
+// length: a composition of public entries, so it computes exactly what the caller would get by chaining them.
+namespace {
+
+constexpr int SR_MODEL = 16000;
+
+// what lies in front of the 16 kHz walk's workspace: both tap tables, the 16 kHz input and output (B rows of L16) and the 16 kHz lengths
+struct SrRegion { float *h_in, *h_out, *x16, *y16; int* len16; };
+
+// places the region at ws (null: sizes it only); returns its size, a multiple of 256 bytes
+size_t sr_region(char* ws, const resample::Ratio& q, int B, long long L16, SrRegion& s) {
+    Walk k;
+    k.dry = ws == nullptr; k.ws = ws; k.cap = SIZE_MAX;
+    const size_t taps = 2 * (size_t)q.half + 1;
+    s.h_in = k.alloc(taps);
+    s.h_out = k.alloc(taps);
+    s.x16 = k.alloc((size_t)B * L16);
+    s.y16 = k.alloc((size_t)B * L16);
+    s.len16 = k.alloc<int>(B);
+    return (k.top + 255) & ~(size_t)255;
+}
+
+// sr -> 16 kHz ratio and the 16 kHz length ceil(L up / down); 0, or -1 with the message set
+int sr_geom(int sr, long long L, long long max16, resample::Ratio& q, long long& L16, const char* who) {
+    if (resample::ratio(sr, SR_MODEL, q, who) != 0) return -1;
+    CMGAN_REQUIRE(L > 0, "%s: L must be positive (L=%lld)", who, L);
+    L16 = (L * q.up + q.down - 1) / q.down;
+    CMGAN_REQUIRE(L16 <= max16, "%s: L=%lld samples at %d Hz are %lld at 16 kHz; at most %lld", who, L, sr, L16, max16);
+    return 0;
+}
+
+}  // namespace
+
+CMGAN_API long long cmgan_enhance_sr_workspace_bytes(int B, int L, int sr, int cut_len, int precision) {
+    if (sr == SR_MODEL) return cmgan_enhance_workspace_bytes(B, L, cut_len, precision);
+    const char* who = "cmgan_enhance_sr_workspace_bytes";
+    if (precision != 0 && precision != 1) { cmgan_set_error("%s: precision must be 0 (fp32) or 1 (tf32)", who); return -1; }
+    resample::Ratio q;
+    long long L16;
+    EnhanceGeom g;
+    if (sr_geom(sr, L, INT32_MAX, q, L16, who) != 0 || enhance_geom(B, (int)L16, cut_len, false, false, g, who) != 0) return -1;
+    SrRegion s;
+    return (long long)sr_region(nullptr, q, B, L16, s) + enhance_bytes(B, (int)L16, g, precision);
+}
+
+CMGAN_API int cmgan_enhance_sr(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int sr, int cut_len, float* out,
+                               long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream) {
+    if (sr == SR_MODEL) return cmgan_enhance(params, wav, ldw, B, L, lengths, cut_len, out, ldo, workspace, workspace_bytes, precision, stream);
+    const char* who = "cmgan_enhance_sr";
+    CMGAN_REQUIRE(params && wav && out && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE(precision == 0 || precision == 1, "%s: precision must be 0 (fp32) or 1 (tf32)", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    resample::Ratio q;
+    long long L16;
+    EnhanceGeom g;
+    if (sr_geom(sr, L, INT32_MAX, q, L16, who) != 0 || enhance_geom(B, (int)L16, cut_len, lengths != nullptr, false, g, who) != 0) return -1;
+    CMGAN_REQUIRE(ldw >= L && ldo >= L, "%s: row strides must cover a clip (L=%d ldw=%lld ldo=%lld)", who, L, ldw, ldo);
+    const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + (B - 1) * ldw + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + (B - 1) * ldo + L);
+    CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "%s: wav and out overlap", who);
+    SrRegion s;
+    const size_t region = sr_region(nullptr, q, B, L16, s);
+    const long long need = (long long)region + enhance_bytes(B, (int)L16, g, precision);
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    sr_region(static_cast<char*>(workspace), q, B, L16, s);
+    const cudaStream_t st = (cudaStream_t)stream;
+    int* len16 = lengths ? s.len16 : nullptr;
+    if (cmgan_resample_taps(sr, SR_MODEL, s.h_in, stream) != 0 || cmgan_resample_taps(SR_MODEL, sr, s.h_out, stream) != 0) return -1;
+    if (resample::launch<float>(wav, ldw, B, L, lengths, q.up, q.down, q.half, s.h_in, s.x16, L16, L16, nullptr, len16, st) != 0) return -1;
+    if (cmgan_enhance(params, s.x16, L16, B, (int)L16, len16, cut_len, s.y16, L16, static_cast<char*>(workspace) + region,
+                      workspace_bytes - (long long)region, precision, stream) != 0)
+        return -1;
+    return resample::launch<float>(s.y16, L16, B, L16, len16, q.down, q.up, q.half, s.h_out, out, ldo, L, lengths, nullptr, st);
+}
+
+CMGAN_API long long cmgan_enhance_long_sr_workspace_bytes(long long L, int sr, int cut_len, int max_segments, int precision) {
+    if (sr == SR_MODEL) return cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision);
+    const char* who = "cmgan_enhance_long_sr_workspace_bytes";
+    resample::Ratio q;
+    long long L16;
+    if (sr_geom(sr, L, 1ll << 30, q, L16, who) != 0) return -1;
+    const long long walk = enhance_long_bytes(cut_len, max_segments, precision, who);
+    if (walk < 0) return -1;
+    SrRegion s;
+    return (long long)sr_region(nullptr, q, 1, L16, s) + walk;
+}
+
+CMGAN_API int cmgan_enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int max_segments, float* out,
+                                    void* workspace, long long workspace_bytes, int precision, void* stream) {
+    const char* who = "cmgan_enhance_long_sr";
+    if (sr == SR_MODEL) {
+        CMGAN_REQUIRE(L >= 0 && L <= (1ll << 30), "%s: L=%lld samples; at most 2^30 (18.6 hours at 16 kHz) keeps every sample index in 32 bits", who, L);
+        return cmgan_enhance_long(params, wav, (int)L, cut_len, max_segments, out, workspace, workspace_bytes, precision, stream);
+    }
+    CMGAN_REQUIRE(params && wav && out && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    resample::Ratio q;
+    long long L16;
+    if (sr_geom(sr, L, 1ll << 30, q, L16, who) != 0) return -1;
+    const long long walk = enhance_long_bytes(cut_len, max_segments, precision, who);
+    if (walk < 0) return -1;
+    EnhanceGeom g;
+    if (enhance_geom(1, (int)L16, cut_len, false, true, g, who) != 0) return -1;
+    const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + L);
+    CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "%s: wav and out overlap", who);
+    SrRegion s;
+    const size_t region = sr_region(nullptr, q, 1, L16, s);
+    const long long need = (long long)region + walk;
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    sr_region(static_cast<char*>(workspace), q, 1, L16, s);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (cmgan_resample_taps(sr, SR_MODEL, s.h_in, stream) != 0 || cmgan_resample_taps(SR_MODEL, sr, s.h_out, stream) != 0) return -1;
+    if (resample::launch<float>(wav, L, 1, L, nullptr, q.up, q.down, q.half, s.h_in, s.x16, L16, L16, nullptr, nullptr, st) != 0) return -1;
+    if (cmgan_enhance_long(params, s.x16, (int)L16, cut_len, max_segments, s.y16, static_cast<char*>(workspace) + region,
+                           workspace_bytes - (long long)region, precision, stream) != 0)
+        return -1;
+    return resample::launch<float>(s.y16, L16, 1, L16, nullptr, q.down, q.up, q.half, s.h_out, out, L, L, nullptr, nullptr, st);
 }
 
 // ==================================================================================== training: train-mode (or saving eval-mode) forward, backward

@@ -2,7 +2,8 @@
 
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
-out, and ``cmgan_enhance_long`` runs one clip of any length through a fixed-size workspace, a few folded segments at a time.
+out, and ``cmgan_enhance_long`` runs one clip of any length through a fixed-size workspace, a few folded segments at a time;
+``cmgan_enhance_sr`` / ``cmgan_enhance_long_sr`` run them on clips at any supported sample rate (``sr=``), resampling on the device.
 ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
 parameter and input gradients.  ``cmgan_disc_fwd`` / ``cmgan_disc_bwd`` are the same pair for the metric discriminator (ref: discriminator.py:29-64),
 with the spectral-norm power iteration, parameter gradients through the spectral norm and input gradients.  ``cmgan_gen_wave_fwd`` /
@@ -71,24 +72,29 @@ def tscnet_forward(flat: torch.Tensor, x: torch.Tensor, precision: int = 1, work
     return fr, fi
 
 
-def enhance_workspace_bytes(B: int, L: int, cut_len: int = 16000 * 16, precision: int = 1) -> int:
-    """workspace of ``cmgan_enhance`` for B clips of up to L samples (the same size for the uniform and the ragged call)"""
-    n = lib().cdll.cmgan_enhance_workspace_bytes(B, L, cut_len, precision)
+def enhance_workspace_bytes(B: int, L: int, cut_len: int = 16000 * 16, precision: int = 1, sr: int = signal.SR_MODEL) -> int:
+    """workspace of ``cmgan_enhance`` (``cmgan_enhance_sr`` at another ``sr``) for B clips of up to L samples (the same size for the uniform
+    and the ragged call)"""
+    if sr == signal.SR_MODEL:
+        n = lib().cdll.cmgan_enhance_workspace_bytes(B, L, cut_len, precision)
+    else:
+        n = lib().cdll.cmgan_enhance_sr_workspace_bytes(B, L, sr, cut_len, precision)
     if n < 0:
         raise RuntimeError(lib().cdll.cmgan_last_error().decode())
     return n
 
 
 def enhance(flat: torch.Tensor, wav: torch.Tensor, lengths=None, cut_len: int = 16000 * 16, precision: int = 1, workspace: torch.Tensor = None,
-            out: torch.Tensor = None) -> torch.Tensor:
+            out: torch.Tensor = None, sr: int = signal.SR_MODEL) -> torch.Tensor:
     """``cmgan_enhance``: noisy waveforms (B, L) on the GPU (unit row stride) -> enhanced waveforms in ``out`` (B, L), which is returned.
     ``lengths=None``: every row is a clip of L samples (folded past ``cut_len``, as evaluation.py does).  Otherwise a ragged batch: clip b is
     wav[b, :lengths[b]] (a device int32 (B,) tensor is used as is, anything else goes through torch.as_tensor); out[b, lengths[b]:] is left
-    as it was (zeros when ``out`` is allocated here)."""
+    as it was (zeros when ``out`` is allocated here).  ``sr``: the clips' sample rate; other than 16 kHz, ``cmgan_enhance_sr`` resamples them
+    to 16 kHz, enhances them there (cut_len and the ragged limit count 16 kHz samples) and resamples the result back."""
     assert wav.is_cuda and flat.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2 and wav.stride(1) == 1
     B, L = wav.shape
     if workspace is None:
-        workspace = torch.empty(enhance_workspace_bytes(B, L, cut_len, precision), dtype=torch.uint8, device=wav.device)
+        workspace = torch.empty(enhance_workspace_bytes(B, L, cut_len, precision, sr), dtype=torch.uint8, device=wav.device)
     if out is None:
         out = (torch.empty if lengths is None else torch.zeros)(B, L, device=wav.device)
     assert out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (B, L) and out.stride(1) == 1
@@ -96,8 +102,13 @@ def enhance(flat: torch.Tensor, wav: torch.Tensor, lengths=None, cut_len: int = 
     if lengths is not None:
         lens = torch.as_tensor(lengths, dtype=torch.int32, device=wav.device).reshape(-1).contiguous()
         assert lens.numel() == B, f"lengths has {lens.numel()} entries for a batch of {B}"
-    lib().call("cmgan_enhance", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), cut_len,
-               out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, torch.cuda.current_stream().cuda_stream)
+    stream = torch.cuda.current_stream().cuda_stream
+    if sr == signal.SR_MODEL:
+        lib().call("cmgan_enhance", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), cut_len,
+                   out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, stream)
+    else:
+        lib().call("cmgan_enhance_sr", flat.data_ptr(), wav.data_ptr(), wav.stride(0), B, L, None if lens is None else lens.data_ptr(), sr,
+                   cut_len, out.data_ptr(), out.stride(0), workspace.data_ptr(), workspace.numel(), precision, stream)
     return out
 
 
@@ -109,30 +120,43 @@ def _long_segments(cut_len: int, max_segments, k: int = None) -> int:
     return n if k is None else min(n, k)
 
 
-def enhance_long_workspace_bytes(cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1) -> int:
-    """workspace of ``cmgan_enhance_long``: the same for every clip length"""
-    n = lib().cdll.cmgan_enhance_long_workspace_bytes(cut_len, _long_segments(cut_len, max_segments), precision)
+def enhance_long_workspace_bytes(cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1, sr: int = signal.SR_MODEL,
+                                 L: int = None) -> int:
+    """workspace of ``cmgan_enhance_long``: the same for every clip length.  At another ``sr`` that of ``cmgan_enhance_long_sr`` for a clip of
+    ``L`` samples: the same pass workspace plus the 16 kHz copies of the clip, in and out"""
+    if sr == signal.SR_MODEL:
+        n = lib().cdll.cmgan_enhance_long_workspace_bytes(cut_len, _long_segments(cut_len, max_segments), precision)
+    else:
+        n = lib().cdll.cmgan_enhance_long_sr_workspace_bytes(L, sr, cut_len, _long_segments(cut_len, max_segments), precision)
     if n < 0:
         raise RuntimeError(lib().cdll.cmgan_last_error().decode())
     return n
 
 
 def enhance_long(flat: torch.Tensor, wav: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1,
-                 workspace: torch.Tensor = None, out: torch.Tensor = None) -> torch.Tensor:
+                 workspace: torch.Tensor = None, out: torch.Tensor = None, sr: int = signal.SR_MODEL) -> torch.Tensor:
     """``cmgan_enhance_long``: one noisy clip of any length (1-D, contiguous, on the GPU) -> the enhanced clip in ``out`` (same length), which is
     returned.  The fold's segments (``signal.fold_geometry``) run ``max_segments`` at a time through one workspace whose size does not depend
-    on the length; None = as many as one pass of the longest segments takes (13 at cut_len = 16 s), at most the clip's segment count."""
+    on the length; None = as many as one pass of the longest segments takes (13 at cut_len = 16 s), at most the clip's segment count.
+    ``sr``: the clip's sample rate; other than 16 kHz, ``cmgan_enhance_long_sr`` resamples it to 16 kHz in the workspace, runs the passes there
+    (cut_len counts 16 kHz samples) and resamples the result back."""
     assert wav.is_cuda and flat.is_cuda and wav.dtype == torch.float32 and wav.dim() == 1 and wav.is_contiguous()
     L = wav.numel()
-    k, _ = signal.fold_geometry(L, cut_len)
+    L16 = L if sr == signal.SR_MODEL else signal.resampled_length(L, sr, signal.SR_MODEL)
+    k, _ = signal.fold_geometry(L16, cut_len)
     n = _long_segments(cut_len, max_segments, k)
     if workspace is None:
-        workspace = torch.empty(enhance_long_workspace_bytes(cut_len, n, precision), dtype=torch.uint8, device=wav.device)
+        workspace = torch.empty(enhance_long_workspace_bytes(cut_len, n, precision, sr, L), dtype=torch.uint8, device=wav.device)
     if out is None:
         out = torch.empty(L, device=wav.device)
     assert out.is_cuda and out.dtype == torch.float32 and out.dim() == 1 and out.numel() >= L and out.is_contiguous()
-    lib().call("cmgan_enhance_long", flat.data_ptr(), wav.data_ptr(), L, cut_len, n, out.data_ptr(), workspace.data_ptr(), workspace.numel(),
-               precision, torch.cuda.current_stream().cuda_stream)
+    stream = torch.cuda.current_stream().cuda_stream
+    if sr == signal.SR_MODEL:
+        lib().call("cmgan_enhance_long", flat.data_ptr(), wav.data_ptr(), L, cut_len, n, out.data_ptr(), workspace.data_ptr(), workspace.numel(),
+                   precision, stream)
+    else:
+        lib().call("cmgan_enhance_long_sr", flat.data_ptr(), wav.data_ptr(), L, sr, cut_len, n, out.data_ptr(), workspace.data_ptr(),
+                   workspace.numel(), precision, stream)
     return out
 
 

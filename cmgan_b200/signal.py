@@ -323,17 +323,73 @@ def default_pass_rows(k: int, T: int, device) -> int:
     return max(1, min(k, max_pass_rows(T), fit))
 
 
+SR_MODEL = 16000                # the model's sample rate; ``resample`` converts every other supported rate to it and back
+SR_MIN, SR_MAX, MAX_FACTOR = 8000, 192000, 1024
+
+
+def resample_ratio(sr_in: int, sr_out: int) -> Tuple[int, int]:
+    """(up, down) = sr_out / sr_in in lowest terms, as ``cmgan_resample`` takes it: both rates in [8000, 192000] Hz and up, down <= 1024
+    (every standard rate 8, 11.025, 12, 16, 22.05, 24, 32, 44.1, 48, 88.2, 96, 176.4 or 192 kHz to or from 16 kHz).  Raises ValueError
+    otherwise."""
+    for sr in (sr_in, sr_out):
+        if not (isinstance(sr, int) and SR_MIN <= sr <= SR_MAX):
+            raise ValueError(f"sample rates must be integers in [{SR_MIN}, {SR_MAX}] Hz (got {sr_in} -> {sr_out})")
+    g = math.gcd(sr_in, sr_out)
+    up, down = sr_out // g, sr_in // g
+    if max(up, down) > MAX_FACTOR:
+        raise ValueError(f"{sr_in} -> {sr_out} Hz reduces to up={up} down={down}; at most {MAX_FACTOR} each")
+    return up, down
+
+
+def resampled_length(length: int, sr_in: int, sr_out: int) -> int:
+    """ceil(length up / down): the samples ``resample`` makes of ``length``"""
+    up, down = resample_ratio(sr_in, sr_out)
+    return -(-length * up // down)
+
+
+def _resample_taps(sr_in: int, sr_out: int, dev) -> torch.Tensor:
+    """per-device cache of the taps ``cmgan_resample_taps`` builds (float64 on the device, rounded to fp32 once), the tables the C entries
+    ``cmgan_enhance_sr`` / ``cmgan_enhance_long_sr`` build in their workspace"""
+    n = 2 * 10 * max(resample_ratio(sr_in, sr_out)) + 1
+    return _table(("resample", sr_in, sr_out, dev), (n,), lambda t: call("cmgan_resample_taps", sr_in, sr_out, t))
+
+
 @torch.no_grad()
-def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None) -> torch.Tensor:
+def resample(wav: torch.Tensor, sr_in: int, sr_out: int, lengths=None) -> torch.Tensor:
+    """scipy.signal.resample_poly(wav, up, down) along the last axis on the GPU (``cmgan_resample``): (B, L) or (L,) float32 -> (B, n) or
+    (n,), n = ceil(L up / down), up / down = sr_out / sr_in in lowest terms.  ``lengths`` (B,): a ragged batch, row b is wav[b, :lengths[b]]
+    and gets out[b, :ceil(lengths[b] up / down)] (zeros after); a device int32 tensor is used as is."""
+    assert wav.is_cuda and wav.dtype == torch.float32 and wav.dim() in (1, 2) and wav.stride(-1) == 1
+    x = wav if wav.dim() == 2 else wav[None]
+    B, L = x.shape
+    n = resampled_length(L, sr_in, sr_out)
+    y = (torch.empty if lengths is None else torch.zeros)(B, n, device=wav.device)
+    lens = None
+    if lengths is not None:
+        lens = torch.as_tensor(lengths, dtype=torch.int32, device=wav.device).reshape(-1).contiguous()
+        assert lens.numel() == B, f"lengths has {lens.numel()} entries for a batch of {B}"
+    ldx = x.stride(0) if B > 1 else L           # a single row may carry any stride along its size-1 batch axis
+    call("cmgan_resample", x, ldx, B, L, lens, sr_in, sr_out, _resample_taps(sr_in, sr_out, wav.device), y, y.stride(0))
+    return y if wav.dim() == 2 else y[0]
+
+
+@torch.no_grad()
+def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, sr: int = SR_MODEL) -> torch.Tensor:
     """evaluation.enhance_one_track between load and save (ref: evaluation.py:21-53) on the GPU: (1, L) -> (L,), for a clip of any length.
     The clip is folded as ``fold_geometry`` says; its k segments run through the model ``max_segments`` at a time, all scaled by the whole
     clip's RMS.  Segments share nothing else, so every pass computes what the single-batch fold computes for its rows.  The default
     (``default_pass_rows``) is one pass of all k rows, the reference's batch, when they fit under 2^31, and otherwise as many rows as fit in
     the free device memory (about 5.2 MB per frame in tf32, 9 MB in fp32: 5 rows of 16 s segments in tf32 on an idle 80 GB H100).
-    ``module_abi.enhance_long`` runs the same passes in a fixed workspace (19.8 GB for 13 rows at cut_len = 16 s, tf32)."""
+    ``module_abi.enhance_long`` runs the same passes in a fixed workspace (19.8 GB for 13 rows at cut_len = 16 s, tf32).
+    ``sr``: the clip's sample rate (``resample_ratio`` lists the supported ones).  Other than 16 kHz, the clip is resampled to 16 kHz, enhanced
+    as above (cut_len counts 16 kHz samples) and resampled back, cut to its length: what ``cmgan_enhance_sr`` computes."""
     assert noisy.dim() == 2 and noisy.shape[0] == 1
     if max_segments is not None and max_segments <= 0:
         raise ValueError(f"max_segments must be positive (max_segments={max_segments})")
+    if sr != SR_MODEL:
+        length = noisy.size(-1)
+        est = enhance(model, resample(noisy.contiguous(), sr, SR_MODEL), cut_len, max_segments)
+        return resample(est, SR_MODEL, sr)[:length]
     noisy = noisy.contiguous()
     length = noisy.size(-1)
     k, S = fold_geometry(length, cut_len)
@@ -373,15 +429,20 @@ def ragged_padded_length(length: int, cut_len: int = 16000 * 16) -> int:
 
 
 @torch.no_grad()
-def enhance_ragged(model, waves: Sequence[torch.Tensor], cut_len: int = 16000 * 16) -> List[torch.Tensor]:
+def enhance_ragged(model, waves: Sequence[torch.Tensor], cut_len: int = 16000 * 16, sr: int = SR_MODEL) -> List[torch.Tensor]:
     """Enhance clips of different lengths in ONE batch: ``waves`` = 1-D float32 CUDA waveforms, each no longer than ``cut_len`` after the
     wrap padding -> the list of enhanced waveforms, each what ``enhance`` returns for that clip alone.
 
     The clips share a (B, T_max) frame grid; clip b occupies its first T_b = padded_b / 100 + 1 frames.  Every stage runs on the ragged
     kernels: RMS scale and wrap + reflect padding per clip length, the framed DFT (per frame), the TSCNet forward with ``frames`` = T_b, the
-    inverse DFT (per frame) and an overlap-add that sums each clip's own frames with its own envelope, then de-normalises."""
+    inverse DFT (per frame) and an overlap-add that sums each clip's own frames with its own envelope, then de-normalises.
+    ``sr``: the clips' common sample rate.  Other than 16 kHz, each clip is resampled to 16 kHz, the 16 kHz clips (each no longer than
+    ``cut_len`` after the wrap padding) are enhanced as above and each result is resampled back, cut to its clip's length."""
     if len(waves) == 0:
         return []
+    if sr != SR_MODEL:
+        est = enhance_ragged(model, [resample(w.contiguous(), sr, SR_MODEL) for w in waves], cut_len)
+        return [resample(e.contiguous(), SR_MODEL, sr)[:w.numel()] for w, e in zip(waves, est)]
     dev = waves[0].device
     for w in waves:
         if not (w.is_cuda and w.dtype == torch.float32 and w.dim() == 1 and w.device == dev):

@@ -1,12 +1,15 @@
 /* Speech enhancement from a non-Python host (plain C99): one noisy mono clip in, the enhanced clip out, through the waveform-level entry
  * cmgan_enhance of libcmgan_b200.so (evaluation.py:21-53 as one call), or through cmgan_enhance_long, which runs a clip of any length a few
- * folded segments at a time in a workspace whose size does not depend on the length.
+ * folded segments at a time in a workspace whose size does not depend on the length; at a sample rate other than 16 kHz through
+ * cmgan_enhance_sr / cmgan_enhance_long_sr, which resample on the device around them.
  *   Build:  gcc -std=c99 -Iinclude examples/c_enhance.c -o c_enhance -Lcmgan_b200 -lcmgan_b200 -Wl,-rpath,$PWD/cmgan_b200
  *           (add -DWITH_CUDA -I/usr/local/cuda/include -L/usr/local/cuda/lib64 -lcudart to enhance a clip).
- *   Run:    c_enhance [params.f32 noisy.f32 enhanced.f32 [precision [cut_len [max_segments]]]]
- *           (max_segments > 0 switches to cmgan_enhance_long with passes of at most that many segments)
+ *   Run:    c_enhance [params.f32 noisy.f32 enhanced.f32 [precision [cut_len [max_segments [sr]]]]]
+ *           (max_segments > 0 switches to cmgan_enhance_long with passes of at most that many segments; sr = the clip's sample rate, 16000
+ *           by default; cut_len counts 16 kHz samples)
+ *           c_enhance sr  only prints the workspace queries, those of the sample-rate entries at sr.
  * params.f32 is a raw little-endian float32 dump of the parameter block (cmgan_b200.module_abi.pack_params(...).cpu().numpy().tofile(path));
- * noisy.f32 / enhanced.f32 are raw little-endian float32 samples at 16 kHz (the reference reads 16-bit wav files and divides by 32768).
+ * noisy.f32 / enhanced.f32 are raw little-endian float32 samples at sr (the reference reads 16-bit wav files and divides by 32768).
  * Without WITH_CUDA only the host-side workspace queries and argument checks run (no GPU needed). */
 #include <stdio.h>
 #include <stdlib.h>
@@ -45,10 +48,17 @@ int main(int argc, char** argv) {
     }
     if (cmgan_enhance_long_workspace_bytes(16000 * 16, 14, 1) >= 0) { fprintf(stderr, "14 segments of 16 s must be rejected\n"); return 1; }
     printf("rejected max_segments=14: %s\n", cmgan_last_error());
+    /* the sample-rate entries: at 16 kHz the same sizes as above; the long one grows with the clip (its 16 kHz copies, in and out) */
+    const int qsr = argc == 2 ? atoi(argv[1]) : 48000;
+    const long long ws_sr = cmgan_enhance_sr_workspace_bytes(1, qsr, qsr, 16000 * 16, 1);
+    const long long ws_long_sr = cmgan_enhance_long_sr_workspace_bytes(3600LL * qsr, qsr, 16000 * 16, 13, 1);
+    if (ws_sr < 0 || ws_long_sr < 0) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
+    printf("workspace sr=%d uniform B=1 L=%d cut_len=%d tf32: %lld bytes\n", qsr, qsr, 16000 * 16, ws_sr);
+    printf("workspace sr=%d long L=%lld cut_len=%d max_segments=13 tf32: %lld bytes\n", qsr, 3600LL * qsr, 16000 * 16, ws_long_sr);
 #ifdef WITH_CUDA
     if (argc > 3) {
         const int precision = argc > 4 ? atoi(argv[4]) : 1, cut_len = argc > 5 ? atoi(argv[5]) : 16000 * 16;
-        const int max_segments = argc > 6 ? atoi(argv[6]) : 0;
+        const int max_segments = argc > 6 ? atoi(argv[6]) : 0, sr = argc > 7 ? atoi(argv[7]) : 16000;
         const long long total = cmgan_tscnet_param_floats();
         float* hp = (float*)malloc((size_t)total * 4);
         FILE* f = fopen(argv[1], "rb");
@@ -62,8 +72,8 @@ int main(int argc, char** argv) {
         float* hx = (float*)malloc((size_t)L * 4);
         if (L <= 0 || fread(hx, 4, (size_t)L, f) != (size_t)L) { fprintf(stderr, "cannot read %s\n", argv[2]); return 1; }
         fclose(f);
-        const long long ws = max_segments > 0 ? cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision)
-                                              : cmgan_enhance_workspace_bytes(1, L, cut_len, precision);
+        const long long ws = max_segments > 0 ? cmgan_enhance_long_sr_workspace_bytes(L, sr, cut_len, max_segments, precision)
+                                              : cmgan_enhance_sr_workspace_bytes(1, L, sr, cut_len, precision);
         if (ws < 0) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
         float *params, *x, *y;
         void* wsp;
@@ -74,8 +84,8 @@ int main(int argc, char** argv) {
         }
         cudaMemcpy(params, hp, (size_t)total * 4, cudaMemcpyHostToDevice);
         cudaMemcpy(x, hx, (size_t)L * 4, cudaMemcpyHostToDevice);
-        const int rc = max_segments > 0 ? cmgan_enhance_long(params, x, L, cut_len, max_segments, y, wsp, ws, precision, 0)
-                                        : cmgan_enhance(params, x, L, 1, L, NULL, cut_len, y, L, wsp, ws, precision, 0);
+        const int rc = max_segments > 0 ? cmgan_enhance_long_sr(params, x, L, sr, cut_len, max_segments, y, wsp, ws, precision, 0)
+                                        : cmgan_enhance_sr(params, x, L, 1, L, NULL, sr, cut_len, y, L, wsp, ws, precision, 0);
         if (rc) { fprintf(stderr, "%s\n", cmgan_last_error()); return 1; }
         if (cudaMemcpy(hx, y, (size_t)L * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { fprintf(stderr, "device error\n"); return 1; }
         f = fopen(argv[3], "wb");
@@ -85,9 +95,6 @@ int main(int argc, char** argv) {
         cudaFree(params); cudaFree(x); cudaFree(y); cudaFree(wsp);
         free(hp); free(hx);
     }
-#else
-    (void)argc;
-    (void)argv;
 #endif
     return 0;
 }

@@ -270,6 +270,38 @@ int cmgan_enhance(const float* params, const float* wav, long long ldw, int B, i
 long long cmgan_enhance_long_workspace_bytes(int cut_len, int max_segments, int precision);
 int cmgan_enhance_long(const float* params, const float* wav, int L, int cut_len, int max_segments, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
 
+/* ---- sample-rate conversion: scipy.signal.resample_poly(x, up, down) with its default filter, up / down = sr_out / sr_in in lowest terms.
+ * Supported: 8000 <= sr_in, sr_out <= 192000 Hz with up, down <= 1024 -- the standard rates 8, 11.025, 12, 16, 22.05, 24, 32, 44.1, 48, 88.2,
+ * 96, 176.4 and 192 kHz to and from 16 kHz, and most pairs among them (not 11.025 <-> 32 kHz and its multiples, 1280 / 441); any other pair
+ * returns -1 with a message.
+ * cmgan_resample_taps_floats: 2 half + 1, half = 10 max(up, down) (12 801 at 11.025 <-> 16 kHz, the largest).
+ * cmgan_resample_taps: writes the taps h[m] = firwin(2 half + 1, 1 / max(up, down), window=('kaiser', 5.0))[m] * up into h (device, that many
+ *   floats), computed in float64 on the device (sinc times a Kaiser(5) window with a series I0, normalised by its sum) and rounded to fp32 once.
+ * cmgan_resample: x (B, L) with row stride ldx >= L -> y (B, ceil(L up / down)) with row stride ldy >= ceil(L up / down); x and y may not
+ *   overlap; h = the taps of (sr_in, sr_out).  y[b, n] = sum_i x[b, i] h[down n + half - up i] over the i in [0, len_b) the filter reaches
+ *   (zero padding at both ends), summed in increasing i.  lengths == NULL: every len_b = L.  Otherwise device int32[B], clamped to [0, L]:
+ *   row b reads only x[b, :len_b] and writes only y[b, :ceil(len_b up / down)]. */
+int cmgan_resample_taps_floats(int sr_in, int sr_out);
+int cmgan_resample_taps(int sr_in, int sr_out, float* h, void* stream);
+int cmgan_resample(const float* x, long long ldx, int B, long long L, const int* lengths, int sr_in, int sr_out, const float* h, float* y, long long ldy, void* stream);
+
+/* ---- module level, waveform in / waveform out at any supported sample rate sr (the list above): the entries above around the 16 kHz model.
+ * cmgan_enhance_sr: the clips are resampled to 16 kHz into the workspace (L16 = ceil(L 16000 / sr) samples; a ragged batch's 16 kHz lengths
+ *   are computed on the device), cmgan_enhance runs on them in the rest of the workspace, and its 16 kHz output is resampled back into out and
+ *   cut to each clip's length: out[b, :L] (ragged: out[b, :lengths[b]], nothing past it written).  The result is bit for bit cmgan_resample ->
+ *   cmgan_enhance -> cmgan_resample.  The fold, the ragged limit and every rejection of cmgan_enhance apply to L16; cut_len counts 16 kHz
+ *   samples.  Also -1 for an unsupported sr or L16 >= 2^31.
+ * cmgan_enhance_long_sr: the same around cmgan_enhance_long for one clip of L samples at sr; L may pass 2^30 as long as L16 <= 2^30.  The
+ *   workspace is cmgan_enhance_long's pass workspace, whose size does not depend on L, plus the 16 kHz copies of the whole clip, in and out
+ *   (8 bytes per 16 kHz sample: about 460 MB per hour).  Both copies are needed: the wrap padding of the fold reads the clip's head in the
+ *   last pass.  The activations stay bounded by max_segments as in cmgan_enhance_long; only the copies grow with L.
+ * At sr = 16000 each entry is exactly its 16 kHz counterpart (the same launches) and each query returns the same size.  The queries return -1
+ * for any shape their entry rejects.  Allocates nothing, never synchronises, CUDA-graph capturable. */
+long long cmgan_enhance_sr_workspace_bytes(int B, int L, int sr, int cut_len, int precision);
+int cmgan_enhance_sr(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int sr, int cut_len, float* out, long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream);
+long long cmgan_enhance_long_sr_workspace_bytes(long long L, int sr, int cut_len, int max_segments, int precision);
+int cmgan_enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int max_segments, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
