@@ -1,7 +1,7 @@
 // tf32 tensor-core implementation of the row-parallel GEMM contract (gemm_args.h) for sm_90a (H100).
 // Persistent, warp-specialised: each CTA loops over 64-row output tiles through a ring of shared-memory stages.  The accumulator of a
-// tile lives in the registers of one consumer warpgroup (wgmma, M = 64, N = 16 per instruction, K = 8).  Two shapes: 2 CTAs / SM for
-// N <= 64 without a prologue, 1 CTA / SM otherwise.
+// tile lives in the registers of one consumer warpgroup (wgmma, M = 64, K = 8, one instruction per K step over N rounded up to a multiple
+// of 64).  Two shapes: 2 CTAs / SM for N <= 64 without a prologue, 1 CTA / SM otherwise.
 //
 //   warps 0-3  A producers, three modes:
 //              * TMA (cfg.tma = 1): dense row-major A, one thread issues cp.async.bulk.tensor.2d boxes of 64 rows x 32 floats that
@@ -14,7 +14,8 @@
 //              Thread 0 also issues the weight tiles: cp.async.bulk of pre-tiled, pre-swizzled (N x 128 B) blocks, all K chunks once per
 //              CTA when the whole weight fits in shared memory ("resident", every conformer GEMM), else per K chunk through the stage
 //              ring ("streamed", the dilated dense convolutions).
-//   warps 4-7  consumer warpgroup: wgmma over every K chunk of the tile (stage released when its MMAs have retired), then the epilogue
+//   warps 4-7  consumer warpgroup: wgmma over every K chunk of the tile, one wgmma group in flight (a stage is released when the next
+//              chunk's MMAs have been issued and its own have retired), then the epilogue
 //              (compile-time kind): accumulator fragments -> per-warp shared-memory staging -> coalesced float4 rows: bias, dropout,
 //              residual, activation gradients, Swish dual output -> global.
 //
@@ -79,6 +80,52 @@ __global__ void pack_all_kernel(const CmganPackDesc* __restrict__ descs) {
 // (pw = 8 positions along w, ph = 8 lines), fetched through a 4-D tensor map with the tap offset added to the coordinates
 struct TcCfg { int BN, stages, resident, ntiles, tma, nfx, nty, W, H; };
 constexpr int PW = 8, PH = 8;
+
+// the consumer's view of the stage ring: A stages at sA, B stages (streamed) or all K chunks (resident) at sB, full barriers at bars,
+// empty barriers at bars + 8 stages
+struct TileRing { uint32_t sA, sB, bars; int stages, b_tile_bytes, nchunks, resident, lane; };
+
+// every K chunk of one tile into acc, NB 16-column blocks wide (compile time, so the wgmma pipeline is one straight K loop).  One wgmma
+// group stays in flight: chunk q's MMAs are committed before the wait for chunk q - 1, whose stage is then released, so the tensor pipe
+// does not drain at every chunk.  The tile's last group is waited for before returning (the epilogue reads acc).  q counts chunks
+// over the CTA's tiles.  Since chunk q - 1 is released only after full(q) has been waited for, a producer may make full(q) depend on
+// at most the release of chunk q - 2: TMA and register producers wait for the release of chunk q - stages before filling chunk q
+// (stages >= 2); the cp.async producer signals full(q) LAG chunks later, so it needs stages >= LAG + 2.
+template <int NB, int NBMAX>
+__device__ __forceinline__ void tile_mma(float (&acc)[NBMAX][8], const TileRing& r, long& q) {
+    auto empty_bar = [&](long qq) { return r.bars + 8u * (r.stages + (int)(qq % r.stages)); };
+    for (int ch = 0; ch < r.nchunks; ++ch, ++q) {
+        const int s = (int)(q % r.stages);
+        const uint32_t par = (uint32_t)((q / r.stages) & 1);
+        mbar_wait(r.bars + 8u * s, par);
+        const uint64_t adesc = gmma_desc_sw128(r.sA + s * A_STAGE_BYTES);
+        const uint64_t bdesc = gmma_desc_sw128(r.sB + (r.resident ? ch : s) * r.b_tile_bytes);
+        wgmma_fence();
+        mma_chunk<NB, NBMAX>(acc, adesc, bdesc, ch == 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ch > 0) {
+            __syncwarp();
+            if (r.lane == 0) mbar_arrive(empty_bar(q - 1));      // this warp's share of chunk q - 1's stage has been read
+        }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (r.lane == 0) mbar_arrive(empty_bar(q - 1));
+}
+// the same at run time: N rounded up to 64 columns (nw = 1 .. NBMAX / 4 wgmma m64n64 widths), one branch per tile outside the wgmma
+// pipeline.  Each accumulator column is its own dot product, so the columns past N change nothing in the first N, and the epilogue never
+// reads them.  Their B rows (at most 48 rows = 6 KB past the tile, inside the allocation) are whatever lies there: the next ring stage,
+// possibly while TMA or cp.async is writing it, the next resident chunk, or the epilogue staging.  Widths that are not a multiple of 64
+// (an m64n64 block plus an n16 / n32 / n48 tail) would mix accumulator register groups of different sizes across the branches, and
+// ptxas then serializes every wgmma of the kernel (advisory C7511, "insufficient register resources").
+template <int NBMAX, int I = 1>
+__device__ __forceinline__ void tile_mma_nw(int nw, float (&acc)[NBMAX][8], const TileRing& r, long& q) {
+    if constexpr (4 * I <= NBMAX) {
+        if (nw == I) tile_mma<4 * I, NBMAX>(acc, r, q);
+        else tile_mma_nw<NBMAX, I + 1>(nw, acc, r, q);
+    }
+}
 
 // NBMAX: 16-column blocks the accumulator has room for (4: N <= 64, two CTAs per SM; 16: N <= 256)
 template <bool ASYNC_A, int NBMAX, int EPI, bool PATCH>
@@ -155,7 +202,9 @@ __global__ void __launch_bounds__(NTHREADS, NBMAX == 4 ? 2 : 1) gemm_rows_tc_ker
             }
             __syncwarp();
         } else if (ASYNC_A) {
-            const int LAG = stages >= 3 ? 2 : 1;
+            // full(q) is signalled after the wait for the release of chunk q + LAG - stages, which must come before the consumer's
+            // release of chunk q - 1 (one chunk late, see tile_mma): LAG <= stages - 2.  The launcher gives this producer >= 3 stages.
+            const int LAG = stages >= 4 ? 2 : 1;
             long rowoff[4];
             RowInfo ri[4];
             int cur_tile = -1, cur_tap = -1;
@@ -270,21 +319,10 @@ __global__ void __launch_bounds__(NTHREADS, NBMAX == 4 ? 2 : 1) gemm_rows_tc_ker
         else if (EPI == CMGAN_EPI_DSWISH_DROP || EPI == CMGAN_EPI_DBNSWISH) { xbase = g.aux; ldx = g.ldaux; }
         else if (EPI == CMGAN_EPI_ACC) { xbase = g.C; ldx = g.ldc; }
         if (cfg.resident) mbar_wait(bready_bar, 0);
+        const TileRing ring{sA, sB, bars, stages, b_tile_bytes, nchunks, cfg.resident, lane};
         long q = 0;
         for (int lt = 0; lt < my_tiles; ++lt) {
-            for (int ch = 0; ch < nchunks; ++ch, ++q) {
-                const int s = (int)(q % stages);
-                const uint32_t par = (uint32_t)((q / stages) & 1);
-                mbar_wait(full_bar(s), par);
-                const uint64_t adesc = gmma_desc_sw128(sA + s * A_STAGE_BYTES);
-                const uint64_t bdesc = gmma_desc_sw128(sB + (cfg.resident ? ch : s) * b_tile_bytes);
-                wgmma_fence();
-                mma_chunk_n<NBMAX>(nb, acc, adesc, bdesc, ch == 0);
-                wgmma_commit();
-                wgmma_wait<0>();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty_bar(s));          // this warp's share of the stage has been read
-            }
+            tile_mma_nw<NBMAX>((nb + 3) / 4, acc, ring, q);
             // rows of this warp.  Flat tiles: 16 consecutive rows.  Patch tiles (cfg.tma == 2): 2 image lines x 8 positions.
             // Pass ps handles rows 2 ps + rsub; its row index is mfirst + (ps >> 2) * hi_rows + 2 * (ps & 3).
             const int tile = blockIdx.x + lt * gridDim.x;
@@ -499,6 +537,10 @@ int cmgan_gemm_rows_tc_launch(const CmganGemmArgs* a, cudaStream_t st) {
             }
         }
     }
+    // the cp.async producer signals a stage one chunk after loading it and the consumer releases each stage one chunk late: it needs
+    // 3 stages (gemm_rows_tc_kernel, LAG).  The plans above always give it that (two CTAs per SM only with room for 3 stages, one CTA
+    // per SM leaves room for at least 5), so this is a guard, not a path.
+    if (a->pro == CMGAN_PRO_NONE && cfg.tma == 0 && cfg.stages < 3) return 1;
     if (!a->b_packed) {
         long total = (long)nchunks * cfg.BN * KC;
         pack_b_kernel<<<cdiv(total, 256), 256, 0, st>>>(a->B, a->sb_tap, a->sb_k, a->sb_n, a->Cin, a->ntaps, a->N, cfg.BN, a->ws);

@@ -112,23 +112,69 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32_rs(float (&d)[4][8], const u
 }
 #undef CMGAN_D8
 
-// one 32-float K chunk (4 instructions along K) of a 64 x (16 NB) accumulator: both operands K-major SWIZZLE_128B, the B rows 16 at a
-// time (16 rows x 128 B = 2048 bytes = 128 descriptor units).  NB is a compile-time constant, so the accumulators stay in registers.
+// D[64 x 16 W] (+)= A[64 x 8] B[16 W x 8]^T on the accumulator blocks d[0] .. d[W - 1] (W = 4, 8, 12, 16): one wgmma m64n(16 W)k8,
+// whose fragment is the W m64n16k8 fragments side by side.  The A slice is read once for the whole width instead of once per 16 columns.
+#define CMGAN_DJ(b) "+f"(d[b][0]), "+f"(d[b][1]), "+f"(d[b][2]), "+f"(d[b][3]), "+f"(d[b][4]), "+f"(d[b][5]), "+f"(d[b][6]), "+f"(d[b][7])
+template <int W, int NBMAX>
+__device__ __forceinline__ void wgmma_tf32_blocks(float (&d)[NBMAX][8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    static_assert(W <= NBMAX, "accumulator blocks out of range");
+    if constexpr (W == 4) {
+        wgmma_m64n64k8_tf32(*reinterpret_cast<float(*)[4][8]>(&d[0]), adesc, bdesc, accumulate);
+    } else if constexpr (W == 8) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+                     "}, %64, %65, p, 1, 1;\n\t}"
+                     : CMGAN_DJ(0), CMGAN_DJ(1), CMGAN_DJ(2), CMGAN_DJ(3),
+                       CMGAN_DJ(4), CMGAN_DJ(5), CMGAN_DJ(6), CMGAN_DJ(7)
+                     : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    } else if constexpr (W == 12) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {"
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+                     "}, %96, %97, p, 1, 1;\n\t}"
+                     : CMGAN_DJ(0), CMGAN_DJ(1), CMGAN_DJ(2), CMGAN_DJ(3),
+                       CMGAN_DJ(4), CMGAN_DJ(5), CMGAN_DJ(6), CMGAN_DJ(7),
+                       CMGAN_DJ(8), CMGAN_DJ(9), CMGAN_DJ(10), CMGAN_DJ(11)
+                     : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    } else if constexpr (W == 16) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+                     "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+                     "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+                     "}, %128, %129, p, 1, 1;\n\t}"
+                     : CMGAN_DJ(0), CMGAN_DJ(1), CMGAN_DJ(2), CMGAN_DJ(3),
+                       CMGAN_DJ(4), CMGAN_DJ(5), CMGAN_DJ(6), CMGAN_DJ(7),
+                       CMGAN_DJ(8), CMGAN_DJ(9), CMGAN_DJ(10), CMGAN_DJ(11),
+                       CMGAN_DJ(12), CMGAN_DJ(13), CMGAN_DJ(14), CMGAN_DJ(15)
+                     : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    } else {
+        static_assert(W == 4, "no wgmma wrapper for this width");
+    }
+}
+#undef CMGAN_DJ
+
+// one 32-float K chunk (4 K steps of 8) of a 64 x (16 NB) accumulator, both operands K-major SWIZZLE_128B (16 B rows = 2048 bytes =
+// 128 descriptor units): one wgmma m64n(16 NB)k8 per K step, NB = 4, 8, 12 or 16.
 template <int NB, int NBMAX>
 __device__ __forceinline__ void mma_chunk(float (&acc)[NBMAX][8], uint64_t adesc, uint64_t bdesc, bool first) {
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-#pragma unroll
-        for (int j = 0; j < NB; ++j)
-            wgmma_m64n16k8_tf32(acc[j], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(128 * j + 2 * k), (first && k == 0) ? 0u : 1u);
-}
-// the same with NB = nb chosen at run time among 1 .. NBMAX
-template <int NBMAX, int I = 1>
-__device__ __forceinline__ void mma_chunk_n(int nb, float (&acc)[NBMAX][8], uint64_t adesc, uint64_t bdesc, bool first) {
-    if constexpr (I <= NBMAX) {
-        if (nb == I) mma_chunk<I, NBMAX>(acc, adesc, bdesc, first);
-        else mma_chunk_n<NBMAX, I + 1>(nb, acc, adesc, bdesc, first);
-    }
+        wgmma_tf32_blocks<NB, NBMAX>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (first && k == 0) ? 0u : 1u);
 }
 
 }  // namespace cmgan_tc
