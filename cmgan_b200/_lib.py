@@ -44,6 +44,25 @@ class GemmArgs(ctypes.Structure):
     ]
 
 
+class GemmRowsPlan(ctypes.Structure):
+    """Mirror of CmganGemmRowsPlan (cmgan_b200/csrc/gemm_args.h): the launch plan cmgan_gemm_rows_tc_plan reports."""
+    _fields_ = [(n, ctypes.c_int) for n in (
+        "supported", "mode", "tile_rows", "consumers", "threads", "ctas_per_sm", "stages", "resident", "nchunks", "b_tile_bytes",
+        "smem_bytes", "producer_regs", "consumer_regs", "entry_regs", "patch_w", "patch_h")] + [("ntiles", ctypes.c_longlong)]
+
+
+ROWS_MODES = ("register", "cp.async", "tma2d", "patch")       # CmganRowsMode
+
+
+def gemm_rows_plan(args: GemmArgs) -> dict:
+    """launch plan of the tf32 row GEMM for one argument block, computed on the host (no device involved)"""
+    p = GemmRowsPlan()
+    lib().call("cmgan_gemm_rows_tc_plan", ctypes.byref(args), ctypes.byref(p))
+    d = {n: getattr(p, n) for n, _ in GemmRowsPlan._fields_}
+    d["mode"] = ROWS_MODES[p.mode]
+    return d
+
+
 _CTYPE = {
     "int": ctypes.c_int, "long long": ctypes.c_longlong, "unsigned long long": ctypes.c_ulonglong,
     "unsigned int": ctypes.c_uint, "float": ctypes.c_float, "double": ctypes.c_double,

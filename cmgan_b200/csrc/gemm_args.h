@@ -59,6 +59,25 @@ typedef struct CmganGemmArgs {
     int b_packed;              // tf32 path: 1 = ws already holds the re-tiled weight (cmgan_pack_weights after the optimiser step), skip the re-tiling
 } CmganGemmArgs;
 
+// launch plan of the tf32 row GEMM for one argument block (cmgan_gemm_rows_tc_plan; computed on the host, no device involved)
+enum CmganRowsMode {
+    CMGAN_ROWS_REGISTER = 0,   // LDG -> prologue -> st.shared (pro != NONE)
+    CMGAN_ROWS_CPASYNC = 1,    // cp.async row gather (strided / transposed convolutions, epilogues the patch plan does not take)
+    CMGAN_ROWS_TMA2D = 2,      // dense rows, one 2-D TMA box per K chunk
+    CMGAN_ROWS_PATCH = 3       // same-size convolutions, one 4-D TMA box (patch_w x patch_h positions) per tap and K chunk
+};
+typedef struct CmganGemmRowsPlan {
+    int supported;             // 0: the tensor path does not take these arguments (cmgan_gemm_rows_f32 runs the fp32 FFMA kernel)
+    int mode;                  // CmganRowsMode (TMA modes fall back to CMGAN_ROWS_CPASYNC at launch if the driver cannot encode the map)
+    int tile_rows, consumers, threads, ctas_per_sm;
+    int stages, resident, nchunks, b_tile_bytes;
+    int smem_bytes;            // dynamic shared memory per CTA, alignment slack included
+    int producer_regs, consumer_regs;   // per thread after the warpgroup register split; entry_regs = the launch-bounds count
+    int entry_regs;
+    int patch_w, patch_h;      // positions x lines of a patch tile (mode PATCH), else 0
+    long long ntiles;
+} CmganGemmRowsPlan;
+
 // one weight to re-tile for the tensor-core path (cmgan_pack_weights): same meaning as the B / sb_* / Cin / ntaps / N fields above
 typedef struct CmganPackDesc {
     const float* src; float* dst; long long sb_tap, sb_k, sb_n; long long Cin, ntaps, N;

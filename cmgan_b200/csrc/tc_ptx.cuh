@@ -78,6 +78,13 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
     d |= (uint64_t)1 << 62;                             // layout type 1 = SWIZZLE_128B
     return d;
 }
+// warpgroup register re-allocation (sm_90a): every warp of the warpgroup executes it.  dec hands registers back to the CTA's pool, inc
+// waits until the pool has them.  The kernel's entry count (launch bounds) and every split must keep the CTA within the 64 K registers.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -26,6 +26,7 @@ int cmgan_set_tf32_rounding(int on);
 /* ---- dense contractions (replace nn.Linear / nn.Conv1d(k=1) / nn.Conv2d and their autograd; gemm_args.h) */
 int cmgan_gemm_rows_f32(const CmganGemmArgs* a, void* stream);
 int cmgan_gemm_wgrad_f32(const CmganGemmArgs* a, void* stream);
+int cmgan_gemm_rows_tc_plan(const CmganGemmArgs* a, CmganGemmRowsPlan* out);
 int cmgan_pack_weights(const CmganPackDesc* descs, int n, void* stream);
 int cmgan_pack_weight(const float* src, float* dst, long long sb_tap, long long sb_k, long long sb_n, int Cin, int ntaps, int N, void* stream);
 

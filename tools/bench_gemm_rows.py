@@ -7,8 +7,8 @@ Records every cmgan_gemm_rows_f32 launch of one generator step (B utterances of 
 bench.py's extras leg does, groups the launches by shape class (M, N, K and the launch plan) and replays each class back to back
 between CUDA events.  For each class it prints the calls per step, microseconds per call, TFLOP/s and algorithmic GB/s, and the
 class's own floor: the larger of flops / 495 TFLOP/s and bytes / 3.35 TB/s (H100 SXM data sheet, dense tf32 and HBM3).  The plan
-column mirrors the launch decisions of cmgan_gemm_rows_tc_launch (csrc/gemm_tc.cu): A producer mode, CTAs per SM, tile rows and
-resident or streamed weights.  The card name, power limit and SM clock are printed with the numbers.
+column comes from the launch-plan query (csrc/gemm_tc.cu): A producer mode, CTAs per SM, tile rows and consumers, stages and
+resident or streamed weights, as cmgan_gemm_rows_tc_plan reports them.  The card name, power limit and SM clock are printed with the numbers.
 
 --save DIR first replays the recorded calls once, in step order, and writes DIR/checksums.json (a bit-level checksum of each call's
 output right after it ran) and DIR/C_<i>.pt (the whole output tensor of the largest calls), so that two builds can be compared bit
@@ -28,7 +28,6 @@ import torch  # noqa: E402
 PEAK_BYTES = 3.35e12        # H100 SXM HBM3, data sheet
 PEAK_TF32 = 495e12          # H100 SXM dense tf32, data sheet
 CLIP = 32000                # 2 s at 16 kHz (bench.py)
-KC, RESIDENT_MAX, SMEM_LIMIT2, STG_BYTES, A_STAGE = 32, 96 * 1024, 112 * 1024, 17408, 8192
 
 
 def card():
@@ -42,26 +41,24 @@ def card():
 
 
 def plan(a):
-    """launch plan of one call, mirroring cmgan_gemm_rows_tc_launch"""
-    from cmgan_b200 import ops
-    N, ntaps = a.N, a.ntaps
-    nchunks = (a.Cin // KC) * ntaps
-    b_tile = N * KC * 4
-    resident = nchunks * b_tile <= RESIDENT_MAX
-    per_stage = A_STAGE + (0 if resident else b_tile)
-    fixed = 1024 + STG_BYTES + 256 + (nchunks * b_tile if resident else 0)
-    ctas = 2 if (a.pro == ops.PRO_NONE and N <= 64 and fixed + 3 * per_stage <= SMEM_LIMIT2) else 1
-    same_off = all(a.tap_off[t] == a.tap_off[0] for t in range(ntaps))
-    if a.pro != ops.PRO_NONE:
-        mode = "register"
-    elif (a.epi in (ops.EPI_NONE, ops.EPI_ACC) and a.conv and a.mul_y == 1 and a.mul_x == 1 and a.div_y == 1 and a.div_x == 1
-          and a.OH == a.IH and a.OW == a.IW and same_off and a.M % (a.OH * a.OW) == 0):
-        mode = "patch8x8"
-    elif not a.conv and ntaps == 1:
-        mode = "tma2d"
-    else:
-        mode = "cp.async"
-    return f"{mode}/{ctas}cta/64row/{'resident' if resident else 'streamed'}"
+    """launch plan of one call, as cmgan_gemm_rows_tc_plan reports it"""
+    from cmgan_b200._lib import gemm_rows_plan
+    p = gemm_rows_plan(a)
+    if not p["supported"]:
+        return "fp32 FFMA"
+    mode = f"patch{p['patch_w']}x{p['patch_h']}" if p["mode"] == "patch" else p["mode"]
+    return (f"{mode}/{p['ctas_per_sm']}cta/{p['tile_rows']}row x{p['consumers']}/{p['stages']}st/"
+            f"{'resident' if p['resident'] else 'streamed'}")
+
+
+# CmganGemmArgs fields the launch plan depends on (--save writes them for every call, tests/golden/gemm_rows_step_calls.json keeps them)
+PLAN_FIELDS = ("M", "N", "Cin", "ntaps", "lda", "conv", "OH", "OW", "IH", "IW", "mul_y", "mul_x", "div_y", "div_x", "pro", "epi")
+
+
+def plan_fields(a):
+    d = {f: getattr(a, f) for f in PLAN_FIELDS}
+    d["tap_off"] = [a.tap_off[t] - a.tap_off[0] for t in range(a.ntaps)]
+    return d
 
 
 def record(batch, dev):
@@ -117,7 +114,8 @@ def main():
             L.call(p[0], ctypes.byref(p[5]), st)
             outs = [t for t in (p[6][2], p[6][10]) if t is not None]
             outs = [t[0] if isinstance(t, tuple) else t for t in outs]
-            sums.append({"i": i, "M": p[1], "N": p[2], "K": p[3], "plan": plan(p[5]), "sum": [checksum(t) for t in outs]})
+            sums.append({"i": i, "M": p[1], "N": p[2], "K": p[3], "plan": plan(p[5]), "args": plan_fields(p[5]),
+                         "sum": [checksum(t) for t in outs]})
             if i in largest:
                 torch.save(outs[0].cpu(), os.path.join(args.save, f"C_{i}.pt"))
         torch.cuda.synchronize()
@@ -157,10 +155,10 @@ def main():
     res = {"batch": args.batch, **card(), "calls_per_step": len(rows), "classes": len(table),
            "all_calls_back_to_back_ms": round(total_ms, 3), "sum_of_classes_ms": round(sum(r["ms_per_step"] for r in table), 3)}
     print(json.dumps(res))
-    hdr = f"{'M':>8} {'N':>4} {'K':>5} {'plan':34} {'calls':>5} {'us/call':>9} {'ms/step':>8} {'TFLOP/s':>8} {'GB/s':>7} {'floor us':>9} {'bound':>5} {'of floor':>8}"
+    hdr = f"{'M':>8} {'N':>4} {'K':>5} {'plan':40} {'calls':>5} {'us/call':>9} {'ms/step':>8} {'TFLOP/s':>8} {'GB/s':>7} {'floor us':>9} {'bound':>5} {'of floor':>8}"
     print(hdr)
     for r in table[:args.top]:
-        print(f"{r['M']:8d} {r['N']:4d} {r['K']:5d} {r['plan']:34} {r['calls']:5d} {r['us_per_call']:9.1f} {r['ms_per_step']:8.3f} "
+        print(f"{r['M']:8d} {r['N']:4d} {r['K']:5d} {r['plan']:40} {r['calls']:5d} {r['us_per_call']:9.1f} {r['ms_per_step']:8.3f} "
               f"{r['TFLOP_per_s']:8.1f} {r['GB_per_s']:7.1f} {r['floor_us']:9.1f} {r['floor_bound']:>5} {r['fraction_of_floor']:8.3f}")
     if args.json:
         with open(args.json, "w") as fh:
