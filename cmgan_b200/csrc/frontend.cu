@@ -102,10 +102,11 @@ __global__ void pad_reflect_kernel(const float* __restrict__ x, long ldx, int L,
 // FOLD (evaluation.py:25-34): every clip has L samples and lens is unused; clip b, wrap-padded with its own head, is cut into segments of
 // S samples, and this launch fills k rows per clip: row b k + r is segment seg0 + r, reflect-padded by 200 on each side (its own edges) and
 // scaled by c[b] -- the rows signal.enhance feeds its DFT after the reshape, without the wrapped copy.  Needs S > 200 and a wrapped length
-// (seg0 + k) S <= 2 L (checked on the host).
+// (seg0 + k) S <= 2 L (checked on the host).  Segment r starts at sample r hop of the wrapped clip: hop = S is the fold, hop < S the
+// overlapping windows of cmgan_enhance_overlap, which need (seg0 + k - 1) hop + S <= 2 L.
 template <bool FOLD>
 __global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, int L, const int* __restrict__ lens, int k, int S, int seg0,
-                                        const float* __restrict__ c, float* __restrict__ xp, int Lp) {
+                                        int hop, const float* __restrict__ c, float* __restrict__ xp, int Lp) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int row = blockIdx.y;
     if (i >= Lp) return;
@@ -117,7 +118,7 @@ __global__ void pad_wrap_reflect_kernel(const float* __restrict__ x, long ldx, i
         int j = i - NFFT / 2;
         if (j < 0) j = -j;
         if (j >= Lw) j = 2 * (Lw - 1) - j;
-        if (FOLD) j += (seg0 + row - b * k) * Lw;     // segment r starts at sample r S of the wrapped clip
+        if (FOLD) j += (seg0 + row - b * k) * hop;    // segment r starts at sample r hop of the wrapped clip
         if (j >= Lb) j -= Lb;                         // wrap padding: sample Lb + k is sample k
         j = clamp_len(j, Lb - 1);                     // only reachable for lengths the host rejects
         v = __ldg(x + (long)b * ldx + j) * (c ? c[b] : 1.f);
@@ -270,6 +271,41 @@ __global__ void ola_ragged_kernel(const float* __restrict__ frames, int T, const
         if (c_div) s /= c_div[b];
     }
     y[(long)b * ldy + n] = s;
+}
+
+// ------------------------------------------------------------------ crossfade of overlapping windows (cmgan_enhance_overlap)
+// w[m] = fp32(sin^2(pi (m + 0.5) / (2 O))), m < O: float64 on the device, each step an explicit _rn intrinsic (the order numpy evaluates
+// np.sin(np.pi * (m + 0.5) / (2 * O)) ** 2 in), rounded to fp32 once.  w[m] + w[O - 1 - m] = 1 in exact arithmetic.
+__global__ void crossfade_table_kernel(float* __restrict__ w, int O) {
+    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < O; m += gridDim.x * blockDim.x) {
+        const double s = sin(__ddiv_rn(__dmul_rn(3.141592653589793, __dadd_rn((double)m, 0.5)), (double)(2 * O)));
+        w[m] = (float)__dmul_rn(s, s);
+    }
+}
+
+// Windows j0 .. j0 + rows - 1 of k, window j covering samples [j H, j H + S), H = S - O, staged as y (rows, S).  For n in [n0, n1), with
+// j = min(n / H, k - 1) and m = n - j H:
+//   j >= 1 and m < O:  out[n] = fp32(w[O - 1 - m] y_{j-1}[m + H]) + fp32(w[m] y_j[m])    (two rounded products, a rounded sum: no FMA)
+//   otherwise:         out[n] = y_j[m]
+// The pass's range is n0 = j0 H up to n1 = L after the last window, else n1 = (j0 + rows) H + O: the first O samples of the next window
+// j0 + rows, where only its predecessor's half, fp32(w[O - 1 - m] y_{j0+rows-1}[m + H]), is known.  That half is written into out and the
+// next pass adds its own to it (its first window finds y_{j-1} there), so nothing is carried outside out.
+__global__ void crossfade_kernel(const float* __restrict__ y, int rows, int j0, int k, int S, int O, const float* __restrict__ w,
+                                 float* __restrict__ out, int n0, int n1) {
+    const int n = n0 + blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= n1) return;
+    const int H = S - O;
+    const int j = min(n / H, k - 1), m = n - j * H, r = j - j0;
+    if (r == rows) {                                            // the next pass's first window: hand on the predecessor's half
+        out[n] = __fmul_rn(__ldg(w + O - 1 - m), __ldg(y + (long)(r - 1) * S + m + H));
+        return;
+    }
+    float v = __ldg(y + (long)r * S + m);
+    if (j >= 1 && m < O) {
+        const float a = r > 0 ? __fmul_rn(__ldg(w + O - 1 - m), __ldg(y + (long)(r - 1) * S + m + H)) : out[n];
+        v = __fadd_rn(a, __fmul_rn(__ldg(w + m), v));
+    }
+    out[n] = v;
 }
 
 // gradient of overlap-add: dframes[b, t, k] = dy[b, 100 t + k - 200] / env (zero outside the trimmed range)
@@ -618,14 +654,15 @@ int cmgan_rms_scale_frames(const float* x, long long ldx, int B, int L, const in
     return cmgan_check_launch("rms_scale_kernel");
 }
 
-int cmgan_pad_wrap_reflect_fold(const float* x, long long ldx, int B, int L, int k, int S, int seg0, const float* c, float* xp, int Lp,
-                                cudaStream_t st) {
-    CMGAN_REQUIRE(x && xp && k > 0 && seg0 >= 0 && S > NFFT / 2 && Lp >= S + NFFT && (long long)(seg0 + k) * S <= 2LL * L,
-                  "cmgan_pad_wrap_reflect_fold: need S > 200, Lp >= S + 400 and (seg0 + k) S <= 2 L (L=%d k=%d S=%d seg0=%d Lp=%d)", L, k, S,
-                  seg0, Lp);
+int cmgan_pad_wrap_reflect_fold(const float* x, long long ldx, int B, int L, int k, int S, int seg0, int hop, const float* c, float* xp,
+                                int Lp, cudaStream_t st) {
+    CMGAN_REQUIRE(x && xp && k > 0 && seg0 >= 0 && S > NFFT / 2 && hop > 0 && hop <= S && Lp >= S + NFFT &&
+                      (long long)(seg0 + k - 1) * hop + S <= 2LL * L,
+                  "cmgan_pad_wrap_reflect_fold: need S > 200, 0 < hop <= S, Lp >= S + 400 and (seg0 + k - 1) hop + S <= 2 L (L=%d k=%d S=%d "
+                  "seg0=%d hop=%d Lp=%d)", L, k, S, seg0, hop, Lp);
     if (B == 0) return 0;
     dim3 grid(cdiv(Lp, 256), B * k);
-    pad_wrap_reflect_kernel<true><<<grid, 256, 0, st>>>(x, ldx, L, nullptr, k, S, seg0, c, xp, Lp);
+    pad_wrap_reflect_kernel<true><<<grid, 256, 0, st>>>(x, ldx, L, nullptr, k, S, seg0, hop, c, xp, Lp);
     return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 
@@ -670,7 +707,7 @@ CMGAN_API int cmgan_pad_wrap_reflect_ragged(const float* x, long long ldx, int B
                   "cmgan_pad_wrap_reflect_ragged: need Lp >= ceil(L / 100) * 100 + 400 (L=%d Lp=%d)", L, Lp);
     if (B == 0) return 0;
     dim3 grid(cdiv(Lp, 256), B);
-    pad_wrap_reflect_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, 1, 0, 0, c, xp, Lp);
+    pad_wrap_reflect_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, L, lengths, 1, 0, 0, 0, c, xp, Lp);
     return cmgan_check_launch("pad_wrap_reflect_kernel");
 }
 
@@ -714,6 +751,27 @@ CMGAN_API int cmgan_ola(const float* frames, int B, int T, const float* inv_env,
     dim3 grid(cdiv((long)HOP * (T - 1), 256), B);
     ola_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, inv_env, c_div, y, ldy, 1, 0);
     return cmgan_check_launch("ola_kernel");
+}
+
+CMGAN_API int cmgan_crossfade_table(float* w, int overlap, void* stream) {
+    CMGAN_REQUIRE(w && overlap > 0, "cmgan_crossfade_table: need w and overlap > 0 (overlap=%d)", overlap);
+    crossfade_table_kernel<<<cdiv(overlap, 256), 256, 0, (cudaStream_t)stream>>>(w, overlap);
+    return cmgan_check_launch("crossfade_table_kernel");
+}
+
+CMGAN_API int cmgan_crossfade(const float* y, int rows, int j0, int k, int S, int overlap, const float* w, float* out, long long L, void* stream) {
+    CMGAN_REQUIRE(y && w && out, "cmgan_crossfade: null pointer");
+    CMGAN_REQUIRE(overlap > 0 && 2LL * overlap <= S, "cmgan_crossfade: need 0 < overlap <= S / 2 (S=%d overlap=%d)", S, overlap);
+    CMGAN_REQUIRE(rows > 0 && j0 >= 0 && (long long)j0 + rows <= k, "cmgan_crossfade: need rows > 0 and 0 <= j0, j0 + rows <= k (rows=%d j0=%d k=%d)",
+                  rows, j0, k);
+    const long long H = S - overlap;
+    const long long lo = k == 1 ? 1 : (k - 1) * H + overlap;
+    CMGAN_REQUIRE(L <= (1LL << 30) && L >= lo && L <= (k - 1) * H + S,
+                  "cmgan_crossfade: L=%lld must lie in [%lld, (k - 1) H + S = %lld] (the last window's crossfade inside the clip) and be at most "
+                  "2^30 (k=%d H=%lld S=%d)", L, lo, (k - 1) * H + S, k, H, S);
+    const long long n0 = (long long)j0 * H, n1 = j0 + rows == k ? L : (j0 + rows) * H + overlap;
+    crossfade_kernel<<<cdiv(n1 - n0, 256), 256, 0, (cudaStream_t)stream>>>(y, rows, j0, k, S, overlap, w, out, (int)n0, (int)n1);
+    return cmgan_check_launch("crossfade_kernel");
 }
 
 CMGAN_API int cmgan_ola_ragged(const float* frames, int B, int T, const int* tlen, const float* inv_env, const float* inv_tail, const float* c_div,

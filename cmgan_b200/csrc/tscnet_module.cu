@@ -599,10 +599,51 @@ int enhance_geom(int B, int L, int cut_len, bool ragged, bool extend, EnhanceGeo
     return 0;
 }
 
+// The overlapping windows of cmgan_enhance_overlap (signal.overlap_geometry restates it), one clip of L samples, padded = ceil(L / 100) * 100,
+// S_max = 100 floor(cut_len / 100).  Needs overlap O a multiple of 100 with 100 <= O and 2 O <= S_max, cut_len >= 300, L > 200 and
+// padded - L <= L.
+//   padded <= S_max: one window of S = padded samples, the one-segment case of cmgan_enhance_long (h = S).
+//   otherwise: S = S_max, hop h = S - O, k = 1 + ceil((padded - S) / h) windows, window j covering [j h, j h + S) of the clip wrap-padded with
+//   its own head to Lw = (k - 1) h + S; needs Lw - L <= L.
+// 0, or -1 with the message set.
+int overlap_geom(int L, int cut_len, int overlap, EnhanceGeom& g, int& h, const char* who) {
+    CMGAN_REQUIRE(cut_len >= 3 * HOP, "%s: cut_len=%d gives windows of at most %d samples; a window needs more than 200", who, cut_len,
+                  cut_len / HOP * HOP);
+    const int smax = cut_len / HOP * HOP;
+    CMGAN_REQUIRE(overlap >= HOP && overlap % HOP == 0 && 2LL * overlap <= smax,
+                  "%s: overlap=%d must be a multiple of 100 with 100 <= overlap <= %d (half of the %d-sample windows at cut_len=%d)", who, overlap,
+                  smax / 2, smax, cut_len);
+    CMGAN_REQUIRE(L > NFFT / 2, "%s: L=%d samples; a clip needs more than the 200-sample reflect padding of the STFT", who, L);
+    const long long padded = ((long long)L + HOP - 1) / HOP * HOP;
+    CMGAN_REQUIRE(padded - L <= L, "%s: wrap padding L=%d to %lld is longer than the clip", who, L, padded);
+    long long k = 1, S = padded, H = padded;
+    if (padded > smax) {
+        S = smax;
+        H = S - overlap;
+        k = 1 + (padded - S + H - 1) / H;
+        CMGAN_REQUIRE((k - 1) * H + S - L <= L, "%s: wrap padding L=%d to %lld windows of %lld samples at hop %lld is longer than the clip", who,
+                      L, k, S, H);
+    }
+    g.k = (int)k;
+    g.S = (int)S;
+    g.T = g.S / HOP + 1;
+    g.rows = g.k;
+    g.pass = g.rows;
+    g.Lp = (g.S + NFFT + HOP - 1) / HOP * HOP;
+    h = (int)H;
+    return 0;
+}
+
+// the crossfade of overlapping windows: overlap O samples, hop S - O
+struct Crossfade { int overlap, hop; };
+
 // The launch sequence of signal.enhance / enhance_ragged around forward(): the STFT tables and the RMS scales of the whole clips, then the
 // rows in passes of g.pass -- padding, DFT, compression, TSCNet, un-compression, inverse DFT, overlap-add into that pass's range of `out`.
 // Several passes only for one clip (B = 1): the segments share nothing but c.
-void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const int* lengths, const EnhanceGeom& g, float* out, long long ldo) {
+// xf (B = 1 only): the rows are overlapping windows, starting xf->hop samples apart; each pass overlap-adds its windows into a staging buffer
+// and cmgan_crossfade joins them into its range of `out`.
+void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const int* lengths, const EnhanceGeom& g, float* out, long long ldo,
+                  const Crossfade* xf = nullptr) {
     const int T = g.T, F = NFEAT;
     float* fwd = r.alloc((size_t)NFFT * 2 * F);
     float* inv = r.alloc((size_t)2 * F * NFFT);
@@ -615,6 +656,8 @@ void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const i
     float* fi = r.alloc((size_t)g.pass * T * F);
     if (r.live()) r.ok(cmgan_stft_tables(fwd, inv, T, env, tail, r.st));
     if (r.live()) r.ok(lengths ? cmgan_rms_scale_frames(wav, ldw, B, L, lengths, c, tlen, r.st) : cmgan_rms_scale(wav, ldw, B, L, c, r.st));
+    float* xw = xf ? r.alloc(xf->overlap) : nullptr;
+    if (xf && r.live()) r.ok(cmgan_crossfade_table(xw, xf->overlap, r.st));
     const size_t mark = r.top;
     const long long Lout = (long long)HOP * (T - 1);        // samples each segment yields
     for (int s0 = 0; s0 < g.rows; s0 += g.pass) {
@@ -626,7 +669,7 @@ void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const i
             float* S = r.alloc((size_t)MT * 2 * F);
             if (r.live())
                 r.ok(lengths ? cmgan_pad_wrap_reflect_ragged(wav, ldw, B, L, lengths, c, xp, g.Lp, r.st)
-                             : cmgan_pad_wrap_reflect_fold(wav, ldw, B, L, kp, g.S, s0, c, xp, g.Lp, r.st));
+                             : cmgan_pad_wrap_reflect_fold(wav, ldw, B, L, kp, g.S, s0, xf ? xf->hop : g.S, c, xp, g.Lp, r.st));
             Gemm dft(xp, HOP, fwd, 0, 2 * F, 1, nullptr, S, 2 * F, MT, 2 * F, NFFT);
             dft.conv(1, T, 1, g.Lp / HOP);
             if (r.live()) r.ok(cmgan_gemm_rows_f32(&dft.a, r.st));          // precision 0 (memset by Gemm): the DFTs stay exact fp32
@@ -644,9 +687,14 @@ void enhance_walk(Run& r, const float* wav, long long ldw, int B, int L, const i
         if (r.live()) r.ok(cmgan_uncompress(fr, fi, (long long)T * F, F, 1, rows, T, U, r.st));
         Gemm idft(U, 2 * F, inv, 0, NFFT, 1, nullptr, frames, NFFT, MT, NFFT, 2 * F);
         if (r.live()) r.ok(cmgan_gemm_rows_f32(&idft.a, r.st));
-        if (r.live())
+        if (xf) {           // the windows' de-normalised outputs, (rows, S) contiguous, then the crossfade into out
+            float* y = r.alloc((size_t)rows * g.S);
+            if (r.live()) r.ok(cmgan_ola_fold(frames, rows, T, rows, env, c, y, 0, rows * g.S, r.st));
+            if (r.live()) r.ok(cmgan_crossfade(y, rows, s0, g.k, g.S, xf->overlap, xw, out, L, r.st));
+        } else if (r.live()) {
             r.ok(lengths ? cmgan_ola_ragged_lengths(frames, B, T, tlen, lengths, L, env, tail, c, out, ldo, r.st)
                          : cmgan_ola_fold(frames, rows, T, kp, env, c, out + s0 * Lout, ldo, (int)(L - s0 * Lout), r.st));
+        }
         r.top = mark;
     }
 }
@@ -861,22 +909,67 @@ CMGAN_API int cmgan_enhance_sr(const float* params, const float* wav, long long 
     return resample::launch<float>(s.y16, L16, B, L16, len16, q.down, q.up, q.half, s.h_out, out, ldo, L, lengths, nullptr, st);
 }
 
-CMGAN_API long long cmgan_enhance_long_sr_workspace_bytes(long long L, int sr, int cut_len, int max_segments, int precision) {
-    if (sr == SR_MODEL) return cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision);
-    const char* who = "cmgan_enhance_long_sr_workspace_bytes";
+// ==================================================================================== one long clip, overlapping windows joined by a crossfade
+// The pass workspace of cmgan_enhance_overlap at 16 kHz: one pass of max_segments windows of S_max samples plus the crossfade table and the
+// staging rows, and never less than cmgan_enhance_long's (the one-window case runs that entry).  Independent of L.
+static long long overlap_bytes(int cut_len, int overlap, int max_segments, int precision, const char* who) {
+    const long long base = enhance_long_bytes(cut_len, max_segments, precision, who);
+    if (base < 0) return -1;
+    EnhanceGeom g;
+    int h;
+    if (overlap_geom(1 << 30, cut_len, overlap, g, h, who) != 0) return -1;          // a clip long enough for windows of S_max samples
+    g.rows = g.pass = max_segments;
+    const Crossfade xf{overlap, h};
+    Run r;
+    r.P = nullptr; r.ws = nullptr; r.dry = true; r.precision = precision; r.st = nullptr;
+    enhance_walk(r, nullptr, g.S, 1, g.S, nullptr, g, nullptr, g.S, &xf);
+    return std::max(base, (long long)r.peak + 256);
+}
+
+// cmgan_enhance_overlap at 16 kHz, overlap > 0; every check before the first launch
+static int enhance_overlap16(const float* params, const float* wav, long long L, int cut_len, int overlap, int max_segments, float* out,
+                             void* workspace, long long workspace_bytes, int precision, void* stream, const char* who) {
+    CMGAN_REQUIRE(params && wav && out && workspace, "%s: null pointer", who);
+    CMGAN_REQUIRE((((uintptr_t)params) & 15) == 0 && (((uintptr_t)workspace) & 255) == 0, "%s: params must be 16-byte, workspace 256-byte aligned", who);
+    CMGAN_REQUIRE(L <= (1 << 30), "%s: L=%lld samples; at most 2^30 (18.6 hours at 16 kHz) keeps every sample index in 32 bits", who, L);
+    const long long need = overlap_bytes(cut_len, overlap, max_segments, precision, who);
+    if (need < 0) return -1;
+    EnhanceGeom g;
+    int h;
+    if (overlap_geom((int)std::max(L, 0LL), cut_len, overlap, g, h, who) != 0) return -1;
+    const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + L);
+    CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "%s: wav and out overlap", who);
+    CMGAN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%lld bytes needed, %lld given)", who, need, workspace_bytes);
+    if (g.k == 1)           // one window: the one-segment case of the long entry, the same launches
+        return cmgan_enhance_long(params, wav, (int)L, cut_len, max_segments, out, workspace, workspace_bytes, precision, stream);
+    g.pass = std::min(max_segments, g.k);
+    const Crossfade xf{overlap, h};
+    cmgan_set_tf32_rounding(precision);       // as cmgan_tscnet_fwd: producers of tensor-core operands round to nearest on store
+    Run r;
+    r.P = params; r.ws = static_cast<char*>(workspace); r.cap = (size_t)workspace_bytes; r.dry = false; r.precision = precision;
+    r.st = (cudaStream_t)stream; r.who = who;
+    enhance_walk(r, wav, L, 1, (int)L, nullptr, g, out, L, &xf);
+    return r.rc;
+}
+
+// One clip at sr: resample to 16 kHz into the workspace, the 16 kHz long walk (overlap 0: cmgan_enhance_long's fold, else the crossfaded
+// windows) on the rest of it, resample back.  sr = 16000 is the 16 kHz walk itself.
+static long long long_sr_bytes(long long L, int sr, int cut_len, int overlap, int max_segments, int precision, const char* who) {
     resample::Ratio q;
-    long long L16;
-    if (sr_geom(sr, L, 1ll << 30, q, L16, who) != 0) return -1;
-    const long long walk = enhance_long_bytes(cut_len, max_segments, precision, who);
-    if (walk < 0) return -1;
+    long long L16 = L;
+    if (sr != SR_MODEL && sr_geom(sr, L, 1ll << 30, q, L16, who) != 0) return -1;
+    const long long walk = overlap == 0 ? enhance_long_bytes(cut_len, max_segments, precision, who)
+                                        : overlap_bytes(cut_len, overlap, max_segments, precision, who);
+    if (walk < 0 || sr == SR_MODEL) return walk;
     SrRegion s;
     return (long long)sr_region(nullptr, q, 1, L16, s) + walk;
 }
 
-CMGAN_API int cmgan_enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int max_segments, float* out,
-                                    void* workspace, long long workspace_bytes, int precision, void* stream) {
-    const char* who = "cmgan_enhance_long_sr";
+static int enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int overlap, int max_segments, float* out,
+                           void* workspace, long long workspace_bytes, int precision, void* stream, const char* who) {
     if (sr == SR_MODEL) {
+        if (overlap != 0)
+            return enhance_overlap16(params, wav, L, cut_len, overlap, max_segments, out, workspace, workspace_bytes, precision, stream, who);
         CMGAN_REQUIRE(L >= 0 && L <= (1ll << 30), "%s: L=%lld samples; at most 2^30 (18.6 hours at 16 kHz) keeps every sample index in 32 bits", who, L);
         return cmgan_enhance_long(params, wav, (int)L, cut_len, max_segments, out, workspace, workspace_bytes, precision, stream);
     }
@@ -885,10 +978,13 @@ CMGAN_API int cmgan_enhance_long_sr(const float* params, const float* wav, long 
     resample::Ratio q;
     long long L16;
     if (sr_geom(sr, L, 1ll << 30, q, L16, who) != 0) return -1;
-    const long long walk = enhance_long_bytes(cut_len, max_segments, precision, who);
+    const long long walk = overlap == 0 ? enhance_long_bytes(cut_len, max_segments, precision, who)
+                                        : overlap_bytes(cut_len, overlap, max_segments, precision, who);
     if (walk < 0) return -1;
     EnhanceGeom g;
-    if (enhance_geom(1, (int)L16, cut_len, false, true, g, who) != 0) return -1;
+    int h;
+    if ((overlap == 0 ? enhance_geom(1, (int)L16, cut_len, false, true, g, who) : overlap_geom((int)L16, cut_len, overlap, g, h, who)) != 0)
+        return -1;
     const uintptr_t w0 = (uintptr_t)wav, w1 = (uintptr_t)(wav + L), o0 = (uintptr_t)out, o1 = (uintptr_t)(out + L);
     CMGAN_REQUIRE(w1 <= o0 || o1 <= w0, "%s: wav and out overlap", who);
     SrRegion s;
@@ -899,10 +995,37 @@ CMGAN_API int cmgan_enhance_long_sr(const float* params, const float* wav, long 
     const cudaStream_t st = (cudaStream_t)stream;
     if (cmgan_resample_taps(sr, SR_MODEL, s.h_in, stream) != 0 || cmgan_resample_taps(SR_MODEL, sr, s.h_out, stream) != 0) return -1;
     if (resample::launch<float>(wav, L, 1, L, nullptr, q.up, q.down, q.half, s.h_in, s.x16, L16, L16, nullptr, nullptr, st) != 0) return -1;
-    if (cmgan_enhance_long(params, s.x16, (int)L16, cut_len, max_segments, s.y16, static_cast<char*>(workspace) + region,
-                           workspace_bytes - (long long)region, precision, stream) != 0)
+    char* ws16 = static_cast<char*>(workspace) + region;
+    const long long bytes16 = workspace_bytes - (long long)region;
+    if ((overlap == 0 ? cmgan_enhance_long(params, s.x16, (int)L16, cut_len, max_segments, s.y16, ws16, bytes16, precision, stream)
+                      : enhance_overlap16(params, s.x16, L16, cut_len, overlap, max_segments, s.y16, ws16, bytes16, precision, stream, who)) != 0)
         return -1;
     return resample::launch<float>(s.y16, L16, 1, L16, nullptr, q.down, q.up, q.half, s.h_out, out, L, L, nullptr, nullptr, st);
+}
+
+CMGAN_API long long cmgan_enhance_long_sr_workspace_bytes(long long L, int sr, int cut_len, int max_segments, int precision) {
+    if (sr == SR_MODEL) return cmgan_enhance_long_workspace_bytes(cut_len, max_segments, precision);
+    return long_sr_bytes(L, sr, cut_len, 0, max_segments, precision, "cmgan_enhance_long_sr_workspace_bytes");
+}
+
+CMGAN_API int cmgan_enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int max_segments, float* out,
+                                    void* workspace, long long workspace_bytes, int precision, void* stream) {
+    return enhance_long_sr(params, wav, L, sr, cut_len, 0, max_segments, out, workspace, workspace_bytes, precision, stream, "cmgan_enhance_long_sr");
+}
+
+CMGAN_API long long cmgan_enhance_overlap_workspace_bytes(long long L, int sr, int cut_len, int overlap, int max_segments, int precision) {
+    const char* who = "cmgan_enhance_overlap_workspace_bytes";
+    CMGAN_REQUIRE(overlap >= 0, "%s: overlap=%d must be 0 (the fold of cmgan_enhance_long) or a positive multiple of 100", who, overlap);
+    if (overlap == 0) return cmgan_enhance_long_sr_workspace_bytes(L, sr, cut_len, max_segments, precision);
+    return long_sr_bytes(L, sr, cut_len, overlap, max_segments, precision, who);
+}
+
+CMGAN_API int cmgan_enhance_overlap(const float* params, const float* wav, long long L, int sr, int cut_len, int overlap, int max_segments, float* out,
+                                    void* workspace, long long workspace_bytes, int precision, void* stream) {
+    const char* who = "cmgan_enhance_overlap";
+    CMGAN_REQUIRE(overlap >= 0, "%s: overlap=%d must be 0 (the fold of cmgan_enhance_long) or a positive multiple of 100", who, overlap);
+    if (overlap == 0) return cmgan_enhance_long_sr(params, wav, L, sr, cut_len, max_segments, out, workspace, workspace_bytes, precision, stream);
+    return enhance_long_sr(params, wav, L, sr, cut_len, overlap, max_segments, out, workspace, workspace_bytes, precision, stream, who);
 }
 
 // ==================================================================================== training: train-mode (or saving eval-mode) forward, backward

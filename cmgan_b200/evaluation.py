@@ -63,15 +63,16 @@ def natural_sorted(names: Iterable[str]) -> List[str]:
 
 @torch.no_grad()
 def enhance_one_track(model, audio_path: str, saved_dir: Optional[str], cut_len: int, n_fft: int = 400, hop: int = 100,
-                      save_tracks: bool = False) -> Tuple[np.ndarray, int]:
+                      save_tracks: bool = False, overlap: int = 0) -> Tuple[np.ndarray, int]:
     """reference evaluation.py:12-58, same arguments and return value ((length,) float32 numpy array, length).  The file may have any
     sample rate ``signal.resample_ratio`` supports: other than 16 kHz it is resampled to 16 kHz on the GPU, enhanced there and resampled back,
-    and the result has (and is saved at) the file's rate and length."""
+    and the result has (and is saved at) the file's rate and length.  ``overlap`` > 0 (16 kHz samples, a multiple of 100): a file longer
+    than ``cut_len`` is cut into overlapping windows joined by a crossfade instead of the reference's fold (``signal.enhance``)."""
     assert n_fft == 400 and hop == 100, "the CUDA front end is specialised for n_fft 400 / hop 100 (the reference's only setting)"
     name = os.path.split(audio_path)[-1]
     noisy, sr = read_wav(audio_path)
     dev = next(model.parameters()).device
-    est = signal.enhance(model, noisy[:1].to(dev), cut_len=cut_len, sr=sr)
+    est = signal.enhance(model, noisy[:1].to(dev), cut_len=cut_len, sr=sr, overlap=overlap)
     est_audio = est.cpu().numpy()
     length = noisy.size(-1)
     assert len(est_audio) == length
@@ -120,9 +121,10 @@ def padding_waste(lengths: Sequence[int], batches: Sequence[Sequence[int]], cut_
 
 
 @torch.no_grad()
-def enhance_files(model, paths: Sequence[str], cut_len: int = SR * 16, max_batch: int = 16) -> Dict[str, np.ndarray]:
+def enhance_files(model, paths: Sequence[str], cut_len: int = SR * 16, max_batch: int = 16, overlap: int = 0) -> Dict[str, np.ndarray]:
     """Enhance many files, packed into ragged batches of up to ``max_batch`` files of different lengths (``plan_batches``); every output
-    equals the per-file result.  Files longer than ``cut_len`` take the reference's folding path one at a time.  Files may have any
+    equals the per-file result.  Files longer than ``cut_len`` take the reference's folding path one at a time, or with ``overlap`` > 0
+    overlapping windows joined by a crossfade (``signal.enhance``); the ragged batches hold one window per file.  Files may have any
     supported sample rate: they are grouped by rate, each group is planned on its 16 kHz lengths (the lengths the model sees) and
     enhanced with ``sr`` = its rate, and every output has its file's rate and length."""
     dev = next(model.parameters()).device
@@ -136,7 +138,7 @@ def enhance_files(model, paths: Sequence[str], cut_len: int = SR * 16, max_batch
         batches, solo = plan_batches(lens16, cut_len, max_batch)
         for i in solo:
             p, w = files[i]
-            out[p] = signal.enhance(model, w[None].to(dev), cut_len=cut_len, sr=sr).cpu().numpy()
+            out[p] = signal.enhance(model, w[None].to(dev), cut_len=cut_len, sr=sr, overlap=overlap).cpu().numpy()
         for part in batches:
             est = signal.enhance_ragged(model, [files[i][1].to(dev) for i in part], cut_len=cut_len, sr=sr)
             for i, e in zip(part, est):

@@ -2,7 +2,8 @@
 
 ``cmgan_tscnet_fwd`` runs TSCNet.forward (inference mode; ref: generator.py:174-196) from one flat parameter block and a caller-owned
 workspace; ``cmgan_enhance`` wraps it in the signal front and back end (ref: evaluation.py:21-53), noisy waveforms in, enhanced waveforms
-out, and ``cmgan_enhance_long`` runs one clip of any length through a fixed-size workspace, a few folded segments at a time;
+out, and ``cmgan_enhance_long`` runs one clip of any length through a fixed-size workspace, a few folded segments at a time
+(``cmgan_enhance_overlap``: overlapping windows joined by a crossfade instead of the fold, ``overlap=``);
 ``cmgan_enhance_sr`` / ``cmgan_enhance_long_sr`` run them on clips at any supported sample rate (``sr=``), resampling on the device.
 ``cmgan_tscnet_fwd_train`` / ``cmgan_tscnet_bwd`` are the generator's train-mode (or saving eval-mode) forward and its backward, with
 parameter and input gradients.  ``cmgan_disc_fwd`` / ``cmgan_disc_bwd`` are the same pair for the metric discriminator (ref: discriminator.py:29-64),
@@ -121,10 +122,14 @@ def _long_segments(cut_len: int, max_segments, k: int = None) -> int:
 
 
 def enhance_long_workspace_bytes(cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1, sr: int = signal.SR_MODEL,
-                                 L: int = None) -> int:
+                                 L: int = None, overlap: int = 0) -> int:
     """workspace of ``cmgan_enhance_long``: the same for every clip length.  At another ``sr`` that of ``cmgan_enhance_long_sr`` for a clip of
-    ``L`` samples: the same pass workspace plus the 16 kHz copies of the clip, in and out"""
-    if sr == signal.SR_MODEL:
+    ``L`` samples: the same pass workspace plus the 16 kHz copies of the clip, in and out.  ``overlap`` > 0: that of
+    ``cmgan_enhance_overlap`` (again independent of L at 16 kHz)"""
+    if overlap != 0:
+        n = lib().cdll.cmgan_enhance_overlap_workspace_bytes(0 if L is None else L, sr, cut_len, overlap, _long_segments(cut_len, max_segments),
+                                                             precision)
+    elif sr == signal.SR_MODEL:
         n = lib().cdll.cmgan_enhance_long_workspace_bytes(cut_len, _long_segments(cut_len, max_segments), precision)
     else:
         n = lib().cdll.cmgan_enhance_long_sr_workspace_bytes(L, sr, cut_len, _long_segments(cut_len, max_segments), precision)
@@ -134,24 +139,29 @@ def enhance_long_workspace_bytes(cut_len: int = 16000 * 16, max_segments: int = 
 
 
 def enhance_long(flat: torch.Tensor, wav: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, precision: int = 1,
-                 workspace: torch.Tensor = None, out: torch.Tensor = None, sr: int = signal.SR_MODEL) -> torch.Tensor:
+                 workspace: torch.Tensor = None, out: torch.Tensor = None, sr: int = signal.SR_MODEL, overlap: int = 0) -> torch.Tensor:
     """``cmgan_enhance_long``: one noisy clip of any length (1-D, contiguous, on the GPU) -> the enhanced clip in ``out`` (same length), which is
     returned.  The fold's segments (``signal.fold_geometry``) run ``max_segments`` at a time through one workspace whose size does not depend
     on the length; None = as many as one pass of the longest segments takes (13 at cut_len = 16 s), at most the clip's segment count.
     ``sr``: the clip's sample rate; other than 16 kHz, ``cmgan_enhance_long_sr`` resamples it to 16 kHz in the workspace, runs the passes there
-    (cut_len counts 16 kHz samples) and resamples the result back."""
+    (cut_len counts 16 kHz samples) and resamples the result back.
+    ``overlap`` > 0 (16 kHz samples): ``cmgan_enhance_overlap``, overlapping windows (``signal.overlap_geometry``) joined by a raised-cosine
+    crossfade instead of the fold, at any ``sr``; ``max_segments`` then counts windows."""
     assert wav.is_cuda and flat.is_cuda and wav.dtype == torch.float32 and wav.dim() == 1 and wav.is_contiguous()
     L = wav.numel()
     L16 = L if sr == signal.SR_MODEL else signal.resampled_length(L, sr, signal.SR_MODEL)
-    k, _ = signal.fold_geometry(L16, cut_len)
+    k = signal.overlap_geometry(L16, cut_len, overlap)[0] if overlap > 0 else signal.fold_geometry(L16, cut_len)[0]
     n = _long_segments(cut_len, max_segments, k)
     if workspace is None:
-        workspace = torch.empty(enhance_long_workspace_bytes(cut_len, n, precision, sr, L), dtype=torch.uint8, device=wav.device)
+        workspace = torch.empty(enhance_long_workspace_bytes(cut_len, n, precision, sr, L, overlap), dtype=torch.uint8, device=wav.device)
     if out is None:
         out = torch.empty(L, device=wav.device)
     assert out.is_cuda and out.dtype == torch.float32 and out.dim() == 1 and out.numel() >= L and out.is_contiguous()
     stream = torch.cuda.current_stream().cuda_stream
-    if sr == signal.SR_MODEL:
+    if overlap != 0:
+        lib().call("cmgan_enhance_overlap", flat.data_ptr(), wav.data_ptr(), L, sr, cut_len, overlap, n, out.data_ptr(), workspace.data_ptr(),
+                   workspace.numel(), precision, stream)
+    elif sr == signal.SR_MODEL:
         lib().call("cmgan_enhance_long", flat.data_ptr(), wav.data_ptr(), L, cut_len, n, out.data_ptr(), workspace.data_ptr(), workspace.numel(),
                    precision, stream)
     else:

@@ -297,6 +297,41 @@ def fold_geometry(length: int, cut_len: int = 16000 * 16) -> Tuple[int, int]:
     return k, S
 
 
+def overlap_geometry(length: int, cut_len: int = 16000 * 16, overlap: int = 16000) -> Tuple[int, int, int]:
+    """(k, S, H): how ``enhance`` with ``overlap`` > 0 cuts a clip of ``length`` samples into k overlapping windows of S samples, H apart
+    (the C entries' ``overlap_geom``).  padded = ceil(length / 100) * 100, S_max = 100 floor(cut_len / 100).
+    The overlap O is a multiple of 100 with 100 <= O and 2 O <= S_max; cut_len >= 300; 200 < length <= 2^30 and padded - length <= length.
+    1. padded <= S_max: one window of S = padded samples (H = S), the one-segment case of the fold.
+    2. otherwise S = S_max, H = S - O, k = 1 + ceil((padded - S) / H); window j covers samples [j H, j H + S) of the clip wrap-padded with
+       its own head to Lw = (k - 1) H + S, which may not add more than the clip's own length.
+    The windows are joined by a raised-cosine crossfade over the first O samples of every window but the first (``enhance``).
+    Raises ValueError for anything the C entry rejects."""
+    smax = cut_len // HOP * HOP
+    if smax < 3 * HOP:
+        raise ValueError(f"cut_len = {cut_len} gives windows of at most {smax} samples; a window needs more than 200")
+    if not (isinstance(overlap, int) and overlap >= HOP and overlap % HOP == 0 and 2 * overlap <= smax):
+        raise ValueError(f"overlap = {overlap} must be a multiple of 100 with 100 <= overlap <= {smax // 2} (half of the {smax}-sample "
+                         f"windows at cut_len = {cut_len})")
+    padded = -(-length // HOP) * HOP
+    if length <= N_FFT // 2 or padded - length > length:
+        raise ValueError(f"a clip of {length} samples is too short for the wrap padding to {padded} and the 200-sample reflect padding")
+    if length > 1 << 30:
+        raise ValueError(f"a clip of {length} samples is longer than 2^30")
+    if padded <= smax:
+        return 1, padded, padded
+    S, H = smax, smax - overlap
+    k = 1 + -(-(padded - S) // H)
+    if (k - 1) * H + S - length > length:
+        raise ValueError(f"a clip of {length} samples is too short for the wrap padding to {k} windows of {S} samples at hop {H}")
+    return k, S, H
+
+
+def crossfade_table(overlap: int, dev) -> torch.Tensor:
+    """w[m] = sin^2(pi (m + 0.5) / (2 overlap)), m < overlap: the fade-in of the crossfade (w[overlap - 1 - m] is the fade-out), built by
+    ``cmgan_crossfade_table`` (float64 on the device, rounded to fp32 once), per-device cache"""
+    return _table(("crossfade", overlap, dev), (overlap,), lambda t: call("cmgan_crossfade_table", t, overlap))
+
+
 MAX_ELEMENTS = 2 ** 31          # the encoder's concat buffer (rows * T * 201 * 320 floats) is indexed with 32-bit element counts
 
 
@@ -374,7 +409,8 @@ def resample(wav: torch.Tensor, sr_in: int, sr_out: int, lengths=None) -> torch.
 
 
 @torch.no_grad()
-def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, sr: int = SR_MODEL) -> torch.Tensor:
+def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments: int = None, sr: int = SR_MODEL,
+            overlap: int = 0) -> torch.Tensor:
     """evaluation.enhance_one_track between load and save (ref: evaluation.py:21-53) on the GPU: (1, L) -> (L,), for a clip of any length.
     The clip is folded as ``fold_geometry`` says; its k segments run through the model ``max_segments`` at a time, all scaled by the whole
     clip's RMS.  Segments share nothing else, so every pass computes what the single-batch fold computes for its rows.  The default
@@ -382,16 +418,25 @@ def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments:
     the free device memory (about 5.2 MB per frame in tf32, 9 MB in fp32: 5 rows of 16 s segments in tf32 on an idle 80 GB H100).
     ``module_abi.enhance_long`` runs the same passes in a fixed workspace (19.8 GB for 13 rows at cut_len = 16 s, tf32).
     ``sr``: the clip's sample rate (``resample_ratio`` lists the supported ones).  Other than 16 kHz, the clip is resampled to 16 kHz, enhanced
-    as above (cut_len counts 16 kHz samples) and resampled back, cut to its length: what ``cmgan_enhance_sr`` computes."""
+    as above (cut_len counts 16 kHz samples) and resampled back, cut to its length: what ``cmgan_enhance_sr`` computes.
+    ``overlap`` > 0 (16 kHz samples): instead of the fold, the clip is cut into overlapping windows (``overlap_geometry``), each processed
+    as a segment of the fold is, and joined by a raised-cosine crossfade (``cmgan_crossfade``), so that no output sample depends on a window
+    edge alone: the launches of ``cmgan_enhance_overlap``, pass by pass.  A clip that fits one window takes the fold's one-segment path."""
     assert noisy.dim() == 2 and noisy.shape[0] == 1
     if max_segments is not None and max_segments <= 0:
         raise ValueError(f"max_segments must be positive (max_segments={max_segments})")
+    if overlap < 0:
+        raise ValueError(f"overlap must be 0 (the fold) or a positive multiple of 100 (overlap={overlap})")
     if sr != SR_MODEL:
         length = noisy.size(-1)
-        est = enhance(model, resample(noisy.contiguous(), sr, SR_MODEL), cut_len, max_segments)
+        est = enhance(model, resample(noisy.contiguous(), sr, SR_MODEL), cut_len, max_segments, overlap=overlap)
         return resample(est, SR_MODEL, sr)[:length]
     noisy = noisy.contiguous()
     length = noisy.size(-1)
+    if overlap > 0:
+        k, S, H = overlap_geometry(length, cut_len, overlap)
+        if k > 1:
+            return _enhance_overlap(model, noisy, k, S, H, overlap, max_segments)
     k, S = fold_geometry(length, cut_len)
     c = rms_scale(noisy)
     if k * S != length:                 # wrap padding with the signal's own head (evaluation.py:25-29)
@@ -412,6 +457,30 @@ def enhance(model, noisy: torch.Tensor, cut_len: int = 16000 * 16, max_segments:
         o0 = s0 * seg_out
         cnt = min(length - o0, m * seg_out)
         out[o0:o0 + cnt] = audio[:cnt]
+    return out
+
+
+def _enhance_overlap(model, noisy: torch.Tensor, k: int, S: int, H: int, O: int, max_segments) -> torch.Tensor:
+    """``enhance`` with k > 1 overlapping windows: the whole clip's RMS scale, the clip wrap-padded with its own head to (k - 1) H + S and
+    viewed as k rows of S samples H apart, then per pass: stft_compress (reflect padding at each window's own edges), the model,
+    uncompress_istft divided by the scale, and ``cmgan_crossfade`` into the pass's range of the output (plus the first half of the next
+    pass's first crossfade)."""
+    length = noisy.size(-1)
+    c = rms_scale(noisy)
+    Lw = (k - 1) * H + S
+    wrapped = torch.cat([noisy, noisy[:, :Lw - length]], dim=-1) if Lw > length else noisy
+    rows = wrapped.as_strided((k, S), (H, 1))
+    w = crossfade_table(O, noisy.device)
+    T = S // HOP + 1
+    n = min(k, max_segments) if max_segments is not None else default_pass_rows(k, T, noisy.device)
+    out = torch.empty(length, device=noisy.device)
+    for s0 in range(0, k, n):
+        m = min(n, k - s0)
+        cb = c.expand(m).contiguous() if m > 1 else c
+        spec = stft_compress(rows[s0:s0 + m], cb).permute(0, 1, 3, 2)
+        fr, fi = model(spec)
+        y = uncompress_istft(fr, fi, cb)
+        call("cmgan_crossfade", y, m, s0, k, S, O, w, out, length)
     return out
 
 

@@ -87,6 +87,16 @@ int cmgan_ola_bwd(const float* dy, long long lddy, int B, int T, const float* in
  * be null.  fwd_basis (400, 402) = [w cos | -w sin]; inv_basis (402, 400) = the one-sided inverse DFT (weights 1, 2, ..., 2, 1; / 400) times
  * the window; inv_env = 1 / overlap-add envelope of T >= 2 frames (100 (T - 1) samples); inv_tail = its last 100 samples for any T >= 3. */
 int cmgan_stft_tables(float* fwd_basis, float* inv_basis, int T, float* inv_env, float* inv_tail, void* stream);
+/* Crossfade of overlapping windows (cmgan_enhance_overlap; signal.enhance with overlap > 0 runs the same launches).
+ * cmgan_crossfade_table: w[m] = sin^2(pi (m + 0.5) / (2 overlap)), m < overlap, computed in float64 on the device and rounded to fp32 once.
+ * cmgan_crossfade: window j of k covers samples [j H, j H + S) of a clip of L samples, H = S - overlap, 0 < overlap <= S / 2; y (rows, S)
+ *   contiguous holds windows j0 .. j0 + rows - 1.  For n with j = min(n / H, k - 1) in that range and m = n - j H: out[n] = fp32(w[overlap - 1 - m]
+ *   y_{j-1}[m + H]) + fp32(w[m] y_j[m]) (two rounded products, a rounded sum) when j >= 1 and m < overlap, else y_j[m].  Unless j0 + rows = k,
+ *   the call also writes the first half fp32(w[overlap - 1 - m] y_{j0+rows-1}[m + H]) of the next window's crossfade into out, and the call for
+ *   windows from j0 + rows on adds its own half to it: call it for j0 = 0, 1, ... in order.  Writes out[j0 H, ...) and never past L; needs
+ *   (k - 1) H + overlap <= L <= (k - 1) H + S (k > 1) and L <= 2^30. */
+int cmgan_crossfade_table(float* w, int overlap, void* stream);
+int cmgan_crossfade(const float* y, int rows, int j0, int k, int S, int overlap, const float* w, float* out, long long L, void* stream);
 
 /* ---- generator head and tails (generator.py:53,126,136-139,150,175-196) */
 int cmgan_head_conv(const float* x, long long sb, long long sc, long long st, long long sf, int B, int T, int F, const float* w, const float* bias, float* out, long long ldo, void* stream);
@@ -302,6 +312,27 @@ long long cmgan_enhance_sr_workspace_bytes(int B, int L, int sr, int cut_len, in
 int cmgan_enhance_sr(const float* params, const float* wav, long long ldw, int B, int L, const int* lengths, int sr, int cut_len, float* out, long long ldo, void* workspace, long long workspace_bytes, int precision, void* stream);
 long long cmgan_enhance_long_sr_workspace_bytes(long long L, int sr, int cut_len, int max_segments, int precision);
 int cmgan_enhance_long_sr(const float* params, const float* wav, long long L, int sr, int cut_len, int max_segments, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
+
+/* ---- module level, ONE clip of any length at any supported sample rate, with overlapping windows joined by a crossfade: no output sample
+ * depends on a window edge alone.  All lengths below count 16 kHz samples; at another sr the clip is resampled to 16 kHz first and back
+ * afterwards, exactly as cmgan_enhance_long_sr does (the workspace holds the same 16 kHz copies).
+ *   overlap = 0: cmgan_enhance_long_sr (at 16 kHz cmgan_enhance_long): the same launches, and the query returns the same size.
+ *   overlap = O > 0: a multiple of 100 with 100 <= O and 2 O <= S_max = 100 floor(cut_len / 100), cut_len >= 300.  With padded =
+ *   ceil(L / 100) * 100 (200 < L <= 2^30, padded - L <= L):
+ *     padded <= S_max: one window of S = padded samples, the one-segment case of cmgan_enhance_long (the same launches);
+ *     otherwise S = S_max, hop H = S - O, k = 1 + ceil((padded - S) / H) windows, window j covering [j H, j H + S) of the clip wrap-padded
+ *     with its own head to Lw = (k - 1) H + S (rejected when Lw - L > L).
+ *   Window j: scaled by the RMS scale c of the WHOLE clip (cmgan_enhance_long's kernel and order), reflect-padded by 200 at its own edges,
+ *   STFT, compression, TSCNet.forward, un-compression, inverse STFT and overlap-add divided by c: y_j, S samples.  The windows are joined by
+ *   cmgan_crossfade with w = cmgan_crossfade_table(O): out[n] = fp32(w[O - 1 - m] y_{j-1}[m + H]) + fp32(w[m] y_j[m]) in the first O samples
+ *   of every window but the first, y_j[m] elsewhere (j = min(n / H, k - 1), m = n - j H).
+ *   The windows run at most max_segments at a time (the 2^31 bound of cmgan_enhance_long: 13 at cut_len = 16 s); the output does not depend
+ *   on max_segments.  At 16 kHz the workspace does not depend on L.  Only wav[:L] is read and only out[:L] written; the ranges may not overlap.
+ * Both return -1 (message in cmgan_last_error; nothing launched) for a bad overlap or cut_len, L out of range, an unsupported sr, null or
+ * misaligned pointers (params 16-byte, workspace 256-byte), max_segments <= 0 or past the 2^31 bound, precision not 0 / 1, overlapping wav /
+ * out, or a workspace smaller than the query.  Allocates nothing, never synchronises, CUDA-graph capturable. */
+long long cmgan_enhance_overlap_workspace_bytes(long long L, int sr, int cut_len, int overlap, int max_segments, int precision);
+int cmgan_enhance_overlap(const float* params, const float* wav, long long L, int sr, int cut_len, int overlap, int max_segments, float* out, void* workspace, long long workspace_bytes, int precision, void* stream);
 
 #ifdef __cplusplus
 }
