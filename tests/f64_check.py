@@ -1,6 +1,6 @@
-"""Shared helpers of the float64 kernel checks (test_gpu_kernels_f64.py, test_gpu_dense_f64.py, test_gpu_tf32_f64.py): guarded device
-buffers, the element-wise bound |got - ref| <= c 2^-24 ref_abs (plus the tf32 form of it), bit-exact comparison, seeded inputs and the
-dropout mask function."""
+"""Shared helpers of the float64 kernel checks (test_gpu_kernels_f64.py, test_gpu_dense_f64.py, test_gpu_tf32_f64.py,
+test_gpu_norms_f64.py): guarded device buffers, the element-wise bound |got - ref| <= c 2^-24 ref_abs (plus the tf32 form of it), bit-exact
+comparison, seeded inputs, the Swish reference with its error terms and the dropout mask function."""
 import math
 
 import numpy as np
@@ -79,6 +79,28 @@ def _close_tf32(got, ref, lim_u, name, where=None):
     _tf32_ok(got if where is None else got.detach().cpu().reshape(ref.shape)[where], name)
     g = got.detach().double().cpu().reshape(ref.shape)
     _close(got, ref, lim_u.cpu().expand(ref.shape) + 2.0 ** 13 * g.abs(), 1, name, where)
+
+
+def _kink_affine(B, C, seed):
+    """per-(b, c) scale and shift with shift = -m0 * scale exactly: scale = k / 16 (k = 8 .. 40) and m0 a multiple of 2^-10 below 8 make
+    m0 * scale exact in float32, so an input equal to m0 gives z = m0 * scale + shift = 0 exactly, in the kernel (fma or not) and in
+    float64 -- a PReLU input exactly on the kink"""
+    g = _gen(seed)
+    scale = torch.randint(8, 41, (B, C), generator=g).float() / 16
+    m0 = torch.round(torch.randn(B, C, generator=g) * 1024).clamp(-8191, 8191) / 1024
+    return scale, -(m0 * scale), m0
+
+
+def _swish_terms(h):
+    """float64 swish, its derivatives, and sigmoidf_'s error (ex2 / rcp approximations and the rounded argument: 8 + 2 |h|, relative)"""
+    s = torch.sigmoid(h)
+    sw = h * s
+    d1 = s * (1 + h * (1 - s))
+    d2 = s * (1 - s) * (2 + h * (1 - 2 * s))
+    se = 8 + 2 * h.abs()
+    # dswishf_ = s (1 + h (1 - s)): s's error through d/ds = 1 + h (1 - 2 s), 1 - s (one unit of 1), h (1 - s), the add and the product
+    d1_err = s * (1 + h * (1 - 2 * s)).abs() * se + s * h.abs() * (2 - s) + 2 * d1.abs()
+    return sw, d1, d2, se, d1_err
 
 
 def _exact(got, ref, name):

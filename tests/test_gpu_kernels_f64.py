@@ -17,7 +17,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64_check import DEV, EPS, NAN, SENT, TAIL, _buf, _cdiv, _close, _exact, _f32, _gen, _mix_seed, _randn, _tail, _unif
+from f64_check import DEV, EPS, NAN, SENT, TAIL, _buf, _cdiv, _close, _close_tf32, _exact, _f32, _gen, _kink_affine, _mix_seed, _randn, _tail, _unif
 from tf32_model import tf32_rna
 
 pytestmark = pytest.mark.gpu
@@ -25,16 +25,6 @@ pytestmark = pytest.mark.gpu
 if torch.cuda.is_available():
     from cmgan_b200 import ops
     from cmgan_b200.ops import call
-
-
-def _kink_affine(B, C, seed):
-    """per-(b, c) scale and shift with shift = -m0 * scale exactly: scale = k / 16 (k = 8 .. 40) and m0 a multiple of 2^-10 below 8 make
-    m0 * scale exact in float32, so an input equal to m0 gives z = m0 * scale + shift = 0 exactly, in the kernel (fma or not) and in
-    float64 -- a PReLU input exactly on the kink"""
-    g = _gen(seed)
-    scale = torch.randint(8, 41, (B, C), generator=g).float() / 16
-    m0 = torch.round(torch.randn(B, C, generator=g) * 1024).clamp(-8191, 8191) / 1024
-    return scale, -(m0 * scale), m0
 
 
 # ================================================================================================ generator output heads
@@ -769,13 +759,15 @@ def test_ola_bwd(B, T):
 
 
 # ================================================================================================ norm backward at the PReLU kink
-@pytest.mark.parametrize("C,layout", [(64, "aligned"), (64, "padded"), (2, "offset"), (256, "aligned")])
-@pytest.mark.parametrize("batch_stats", [1, 0])
-def test_norm_bwd_prelu_kink(C, layout, batch_stats):
-    """cmgan_norm_bwd_reduce + cmgan_norm_bwd_apply with PReLU inputs exactly 0 on every ninth row, for the 128-bit kernels ("aligned",
-    C % 4 == 0) and the scalar ones (leading dimension C + 1, or a base one float past alignment).  Reference in two autograd stages:
-    torch's PReLU on z = x scale + shift (exact in float64, 0 on the kink rows), then InstanceNorm (batch_stats = 1) or an affine map with
-    fixed statistics (batch_stats = 0, eval BatchNorm) from x to z."""
+NORM_BWD_LAYOUTS = [(64, "aligned"), (64, "padded"), (2, "offset"), (256, "aligned")]
+
+
+def _norm_bwd_case(C, layout, batch_stats, act, rnd):
+    """cmgan_norm_bwd_reduce + cmgan_norm_bwd_apply with inputs on the PReLU kink (z exactly 0) on every ninth row, for the 128-bit kernels
+    ("aligned", C % 4 == 0) and the scalar ones (leading dimension C + 1, or a base one float past alignment); act 1 (PReLU) or 0 (none),
+    dx stored as is (rnd 0) or rounded to tf32 (rnd 16).  Reference in two autograd stages: torch's PReLU on z = x scale + shift (exact in
+    float64, 0 on the kink rows; the identity for act 0), then InstanceNorm (batch_stats = 1) or an affine map with fixed statistics
+    (batch_stats = 0, eval BatchNorm) from x to z."""
     G, rows = 2, 300
     ld = C + 1 if layout == "padded" else C
     off = 1 if layout == "offset" else 0
@@ -802,15 +794,18 @@ def test_norm_bwd_prelu_kink(C, layout, batch_stats):
     ds0, dg0, dbt0 = _randn(C, seed=184), _randn(C, seed=185), _randn(C, seed=186)
     S = torch.zeros(G * C * 2, dtype=torch.float64, device=DEV)
     dsl, dg, dbt = _buf(C, ds0), _buf(C, dg0), _buf(C, dbt0)
-    call("cmgan_norm_bwd_reduce", (xb, off), ld, (db_, off), ld, G, rows, C, 1, scd, shd, mud, rsd, C, sld, S, dsl)
-    call("cmgan_norm_bwd_apply", (xb, off), ld, (db_, off), ld, G, rows, C, 1, batch_stats, scd, shd, mud, rsd, C, sld, S, (dxb, off), ld,
-         dg, dbt)
+    call("cmgan_norm_bwd_reduce", (xb, off), ld, (db_, off), ld, G, rows, C, act, scd, shd, mud, rsd, C, sld, S, dsl)
+    call("cmgan_norm_bwd_apply", (xb, off), ld, (db_, off), ld, G, rows, C, act | rnd, batch_stats, scd, shd, mud, rsd, C, sld, S,
+         (dxb, off), ld, dg, dbt)
     # stage 1: torch's PReLU at z (its backward takes the slope at z = 0)
     zl = (x64 * sc.double()[:, None] + sh.double()[:, None]).requires_grad_()
     assert int((zl == 0).sum()) >= G * C * (rows // 9)
     sll = slope.double().requires_grad_()
-    F.prelu(zl.view(G * rows, C), sll).backward(dy.double().view(G * rows, C))
-    g = zl.grad
+    if act:
+        F.prelu(zl.view(G * rows, C), sll).backward(dy.double().view(G * rows, C))
+        g = zl.grad
+    else:
+        g = dy.double()
     # stage 2: z as a function of x with gamma, beta per (group, channel) such that gamma rstd = scale and beta - mean scale = shift
     xl = x64.clone().requires_grad_()
     if batch_stats:
@@ -828,15 +823,38 @@ def test_norm_bwd_prelu_kink(C, layout, batch_stats):
     chain = 64                                        # float rows per thread: 64 (scalar kernels) or 16 (128-bit ones)
     dx_abs = sc.double().abs()[:, None] * (g.abs() + batch_stats * (s1_abs[:, None] + xh_abs * s2_abs[:, None]) / rows)
     # dx: the per-thread float sums behind S, the apply's 6 roundings, the float32 mean / rstd tables against the exact statistics
-    _close(dxv[:, :C].cpu(), xl.grad.view(G * rows, C), dx_abs.view(G * rows, C), chain + 8, f"norm_bwd dx C={C} {layout}")
+    # (rnd 16: plus half a tf32 spacing of the stored value)
+    nm = f"norm_bwd dx C={C} {layout} act={act} rnd={rnd}"
+    if rnd:
+        _close_tf32(dxv[:, :C].cpu(), xl.grad.view(G * rows, C), (chain + 8) * dx_abs.view(G * rows, C), nm)
+    else:
+        _close(dxv[:, :C].cpu(), xl.grad.view(G * rows, C), dx_abs.view(G * rows, C), chain + 8, nm)
     assert (dxv[:, C:].cpu() == SENT).all()
     _tail(dxb, off + G * rows * ld, "norm_bwd dx")
     # dgamma / dbeta: S (per-thread float sums, double beyond), one float atomic per group, the prefill
     _close(dg[:C], dg0.double() + gl.grad.sum(0), dg0.double().abs() + s2_abs.sum(0), chain + G + 4, "norm_bwd dgamma")
     _close(dbt[:C], dbt0.double() + bl.grad.sum(0), dbt0.double().abs() + s1_abs.sum(0), chain + G + 4, "norm_bwd dbeta")
-    # dslope: per-thread float sums, one float atomic per block, the prefill
-    nblk = G * _cdiv(rows, 16 * (256 // max(C // 4, 1)) if (C % 4 == 0 and layout == "aligned") else 64 * (256 // C))
-    _close(dsl[:C], ds0.double() + sll.grad, ds0.double().abs() + (dy.double().abs() * zl.detach().abs()).sum((0, 1)), chain + nblk + 4,
-           "norm_bwd dslope")
+    # dslope: per-thread float sums, one float atomic per block, the prefill; act 0 leaves it alone
+    if act:
+        nblk = G * _cdiv(rows, 16 * (256 // max(C // 4, 1)) if (C % 4 == 0 and layout == "aligned") else 64 * (256 // C))
+        _close(dsl[:C], ds0.double() + sll.grad, ds0.double().abs() + (dy.double().abs() * zl.detach().abs()).sum((0, 1)), chain + nblk + 4,
+               "norm_bwd dslope")
+    else:
+        _exact(dsl[:C], ds0, "norm_bwd dslope (act 0: not written)")
     for t, nm in ((dsl, "dslope"), (dg, "dgamma"), (dbt, "dbeta")):
         _tail(t, C, f"norm_bwd {nm}")
+
+
+@pytest.mark.parametrize("C,layout", NORM_BWD_LAYOUTS)
+@pytest.mark.parametrize("batch_stats", [1, 0])
+def test_norm_bwd_prelu_kink(C, layout, batch_stats):
+    _norm_bwd_case(C, layout, batch_stats, 1, 0)
+
+
+@pytest.mark.parametrize("act,rnd", [(0, 0), (0, 16), (1, 16)])
+@pytest.mark.parametrize("C,layout", NORM_BWD_LAYOUTS)
+@pytest.mark.parametrize("batch_stats", [1, 0])
+def test_norm_bwd_act_rounding(C, layout, batch_stats, act, rnd):
+    """the same backward without an activation (the BatchNorm of the conformer's convolution module) and with dx rounded to tf32 on store
+    (act | 16, the dense blocks' tf32 path)"""
+    _norm_bwd_case(C, layout, batch_stats, act, rnd)

@@ -24,7 +24,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64_check import DEV, EPS, NAN, SENT, U, _buf, _cdiv, _close, _close_tf32, _exact, _f32, _keep, _mix_seed, _randn, _tail
+from f64_check import DEV, EPS, NAN, SENT, U, _buf, _cdiv, _close, _close_tf32, _exact, _f32, _keep, _mix_seed, _randn, _swish_terms, _tail
 from tf32_model import tf32_rna
 
 pytestmark = pytest.mark.gpu
@@ -319,18 +319,6 @@ def _ln_terms(x):
     mean_err = 34 * mabs
     rstd_rel = 24 + 0.5 * (mean_err * U) ** 2 / (var + _f32(EPS)) / U
     return mu, rstd, mean_err, rstd_rel
-
-
-def _swish_terms(h):
-    """float64 swish, its derivatives, and sigmoidf_'s error (ex2 / rcp approximations and the rounded argument: 8 + 2 |h|, relative)"""
-    s = torch.sigmoid(h)
-    sw = h * s
-    d1 = s * (1 + h * (1 - s))
-    d2 = s * (1 - s) * (2 + h * (1 - 2 * s))
-    se = 8 + 2 * h.abs()
-    # dswishf_ = s (1 + h (1 - s)): s's error through d/ds = 1 + h (1 - 2 s), 1 - s (one unit of 1), h (1 - s), the add and the product
-    d1_err = s * (1 + h * (1 - 2 * s)).abs() * se + s * h.abs() * (2 - s) + 2 * d1.abs()
-    return sw, d1, d2, se, d1_err
 
 
 def _ffn_fwd_ref(x, P, m1, m2):
